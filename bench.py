@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- throughput of the MGProto Gaussian-prototype hot path on B200.
+"""bench.py -- throughput of the MGProto Gaussian-prototype hot path on H100.
 
     python bench.py --gpus N --steps K --warmup W            (driver: torchrun for N > 1)
     python bench.py --impl reference ...                     (CPU arm: the reference algorithm on host cores)
@@ -17,16 +17,21 @@ The backbone is outside the path (SURVEY.md section 8) and is not timed.
           (mgproto_b200.pipeline) so that they overlap the neighbouring steps' compute
   roofline  the log-likelihood kernel (mgp_logprob_fwd, [N,P] output: the north-star kernel), timed
           alone with CUDA events: algorithmic bytes 4*(N*D + 2*P*D + N*P) per launch / duration,
-          against MEASURED_PEAKS.json's HBM copy bandwidth (burst figure: kernel timed alone);
+          against MEASURED_PEAKS.json's HBM copy bandwidth if present, else the H100 SXM data sheet's 3.35 TB/s;
           roofline_step_logprob: the variant the labelled step runs (max/arg-max epilogue, log p stays on
-          chip) against the measured dense bf16 tensor peak
+          chip) against the dense bf16 tensor peak (measured, else the data sheet's 989 TFLOP/s)
   cpu_baseline  the UNMODIFIED reference (baseline/_ref, tools/install_reference.py) on the host cores, bounded
           sample; the numpy oracle port only if baseline/_ref is absent
   reference_gpu_eager  the same-box GPU bar: the unmodified reference model.py run eagerly on cuda:0 at the same
           shapes (no_grad forward, train forward+backward, update_GMM), timed beside our stages
 
-Timing: the --steps block is repeated R >= 10 times (each bracketed by CUDA events); `value` uses the MEDIAN block,
-min/max are reported in `timing`.
+Timing: the --steps timed steps run as R = min(--reps, --steps) blocks (each bracketed by CUDA events); `value` uses
+the MEDIAN per-step time over the blocks, min/max are reported in `timing`.
+
+--dump-outputs DIR  after the timed steps, writes what the last timed step computed as float32 .npy files: the
+          logits [B,C,T] the step returns, the loss gradient w.r.t. the input features [B,D,H,W], and the model state
+          the step leaves behind (prototype means [C,K,D], mixture weights [C,C*K]).  Inputs are seeded, so two builds
+          run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -43,7 +48,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 CFG = dict(B=256, C=200, K=10, D=128, H=14, W=14, T=20, cap=800)
-N_ROT = 8   # distinct input batches rotated through (8 x 25.7 MB of features > the 126 MB L2)
+N_ROT = 8   # distinct input batches rotated through (8 x 25.7 MB of features > the 50 MB L2 of the H100)
 
 
 def peaks():
@@ -51,7 +56,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured"
-    return 6650.0, "fallback"
+    return 3350.0, "H100 SXM data sheet"
 
 
 # ------------------------------------------------------------------------------------------ CPU arm
@@ -211,7 +216,7 @@ def cpu_reference_real(n_img, steps, warmup, threads):
 
 
 def reference_gpu_eager(dev, feats, gts, ours):
-    """SURVEY 2b / 8(d): the same-box GPU bar -- the unmodified reference run eagerly on the B200 at the bench
+    """SURVEY 2b / 8(d): the same-box GPU bar -- the unmodified reference run eagerly on the same GPU at the bench
     shapes, stage by stage, beside our own stages (`ours`: dict of callables).  CUDA events, 1 warm-up + 3 timed."""
     import torch
     ref = _import_reference(cpu=False)
@@ -310,7 +315,7 @@ def _config(n_gpus):
                         "rows/class; step = head fwd+bwd + enqueue + update_GMM"
                         % (c["B"], c["B"], c["D"], c["H"], c["W"], c["C"], c["K"], c["D"], c["T"], c["cap"]),
             "global_batch": c["B"] * n_gpus, "parallelism": par,
-            "l2": "inputs rotate through %d distinct batches (%.0f MB) > 126 MB L2; the labelled step keeps log p on chip (no [B,P,HW] intermediate)"
+            "l2": "inputs rotate through %d distinct batches (%.0f MB) > 50 MB L2; the labelled step keeps log p on chip (no [B,P,HW] intermediate)"
                   % (N_ROT, N_ROT * c["B"] * c["D"] * c["H"] * c["W"] * 4 / 1e6)}
 
 
@@ -355,6 +360,14 @@ class ClockSampler:
                 "reasons": reasons, "samples": len(sm), "window": window}
 
 
+def dump_outputs(path, arrays):
+    """--dump-outputs: each tensor as <name>.npy (float32) under `path`."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), t.detach().float().cpu().numpy())
+
+
 def build_model(dev, seed=0):
     import torch
     import torch.nn as nn
@@ -392,7 +405,9 @@ def main():
     ap.add_argument("--no-ref-gpu", action="store_true", help="skip the reference_gpu_eager leg")
     ap.add_argument("--no-ood", action="store_true", help="skip the configs[4] OoD-scoring throughput leg")
     ap.add_argument("--no-graph", action="store_true", help="run the device-resident leg eagerly instead of replaying a CUDA graph")
-    ap.add_argument("--reps", type=int, default=10, help="repetitions of the --steps block (median reported)")
+    ap.add_argument("--reps", type=int, default=10, help="blocks the --steps timed steps are split into (median reported)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (logits, feature gradient, model state) as .npy into DIR")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference_arm(args)
@@ -414,6 +429,9 @@ def main():
     from mgproto_b200 import ops, parallel
     c = CFG
     W = max(3, args.warmup)
+    if args.steps < 1:
+        raise SystemExit("--steps must be >= 1")
+    torch.manual_seed(0)                              # parameters drawn from the global generator are seeded too
     net = build_model(dev)
     net.math_mode = args.math
     if world > 1:
@@ -466,40 +484,50 @@ def main():
         step(feats[i % N_ROT], gts[i % N_ROT])
     barrier()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    R = max(10, args.reps)                        # the --steps block is repeated R times; value = median block
-    blocks = []
+    R = max(1, min(args.reps, args.steps))        # the --steps timed steps run as R blocks; value = median block
+    sizes = [args.steps // R + (1 if r < args.steps % R else 0) for r in range(R)]
+    blocks = []                                   # per-step ms of each block
     host_enq = []
     barrier()
     t_w0 = time.time()
     launches = 0
+    done = 0
+    last_out = None
     for r in range(R):
         l0 = ops.launch_count()
         barrier()
         e0.record()
         t_h0 = time.perf_counter()
-        for i in range(args.steps):
-            step(feats[(r * args.steps + i) % N_ROT], gts[(r * args.steps + i) % N_ROT])
+        for i in range(sizes[r]):
+            last_out = step(feats[(done + i) % N_ROT], gts[(done + i) % N_ROT])
         e1.record()
-        host_enq.append((time.perf_counter() - t_h0) * 1e3)      # host time to ENQUEUE the block (no sync inside)
+        host_enq.append((time.perf_counter() - t_h0) * 1e3 / sizes[r])   # host time to ENQUEUE a step (no sync inside)
         barrier()
-        tm = torch.tensor([e0.elapsed_time(e1)], device=dev)
+        tm = torch.tensor([e0.elapsed_time(e1) / sizes[r]], device=dev)
         if world > 1:
             dist.all_reduce(tm, op=dist.ReduceOp.MAX)
         blocks.append(float(tm))
-        launches = ops.launch_count() - l0
+        launches = (ops.launch_count() - l0) * args.steps // sizes[r]
         if graphed is not None:                      # replays do not pass through the Python launch counter
             launches = graphed.launches * args.steps
+        done += sizes[r]
     t_w1 = time.time()
-    ms = statistics.median(blocks)
+    if args.dump_outputs and rank == 0:
+        last = (done - 1) % N_ROT
+        x_grad = graphed.x_grad if graphed is not None else feats[last].grad
+        dump_outputs(args.dump_outputs, {"logits": last_out, "grad_features": x_grad,
+                                         "prototype_means": net.prototype_means, "mixture_weights": net.last_layer.weight})
+    ms = statistics.median(blocks) * args.steps  # time of the whole --steps window at the median step time
     value = B * world * args.steps / (ms / 1e3)
-    timing = {"reps": R, "block_ms_median": ms, "block_ms_min": min(blocks), "block_ms_max": max(blocks),
-              "value_from": "median block of %d x %d steps, max over ranks per block" % (R, args.steps),
-              "images_per_s_min": B * world * args.steps / (max(blocks) / 1e3),
-              "images_per_s_max": B * world * args.steps / (min(blocks) / 1e3),
+    timing = {"reps": R, "block_ms_median": ms, "block_ms_min": min(blocks) * args.steps,
+              "block_ms_max": max(blocks) * args.steps,
+              "value_from": "median per-step time of %d blocks over %d timed steps, max over ranks per block" % (R, args.steps),
+              "images_per_s_min": B * world / (max(blocks) / 1e3),
+              "images_per_s_max": B * world / (min(blocks) / 1e3),
               "launch": launch_mode,
-              "host_enqueue_ms_median": statistics.median(host_enq),
-              "host_note": "wall time the Python / ctypes side needs to enqueue one block (no synchronisation inside): the "
-                           "step is GPU-bound while this stays below block_ms_median"}
+              "host_enqueue_ms_median": statistics.median(host_enq) * args.steps,
+              "host_note": "wall time the Python / ctypes side needs to enqueue --steps steps (no synchronisation inside): "
+                           "the step is GPU-bound while this stays below block_ms_median"}
 
     # ---- end to end: host buffers in, logits out ---------------------------------------------
     # every step copies its own pinned-host feature batch to the device and reads its logits back to pinned host
@@ -520,19 +548,22 @@ def main():
         sink.wait()
 
     e2e_run(3)
-    e2e_blocks = []
-    for _ in range(5):
+    e2e_blocks = []                               # per-step ms; the --steps steps as up to 5 blocks
+    R2 = min(5, args.steps)
+    for r in range(R2):
+        n2 = args.steps // R2 + (1 if r < args.steps % R2 else 0)
         barrier()
         e0.record()
-        e2e_run(args.steps)
+        e2e_run(n2)
         e1.record()
         barrier()
-        tm = torch.tensor([e0.elapsed_time(e1)], device=dev)
+        tm = torch.tensor([e0.elapsed_time(e1) / n2], device=dev)
         if world > 1:
             dist.all_reduce(tm, op=dist.ReduceOp.MAX)
         e2e_blocks.append(float(tm))
-    e2e_val = B * world * args.steps / (statistics.median(e2e_blocks) / 1e3)
-    timing["e2e_block_ms"] = {"median": statistics.median(e2e_blocks), "min": min(e2e_blocks), "max": max(e2e_blocks)}
+    e2e_val = B * world / (statistics.median(e2e_blocks) / 1e3)
+    timing["e2e_block_ms"] = {"median": statistics.median(e2e_blocks) * args.steps, "min": min(e2e_blocks) * args.steps,
+                              "max": max(e2e_blocks) * args.steps}
     clocks = sampler.stop(t_w0, t_w1) if rank == 0 else None
 
     # ---- roofline of the log-likelihood kernel (timed alone, rank 0) --------------------------
@@ -556,26 +587,20 @@ def main():
         torch.cuda.synchronize()
         t_op = e0.elapsed_time(e1) / reps / 1e3
         abytes = 4.0 * (N * D + 2 * P * D + N * P)
-        # `roofline` describes mgp_logprob_fwd AS CALLED by compute_log_prob (prototype operand pre-pass + the GEMM
-        # kernel; with isotropic sigma the x operand split is fused into the kernel: csrc/logprob_tcz.cu); the kernel
-        # alone (prototype operands pre-staged) is an extra key
+        # `roofline` describes mgp_logprob_fwd AS CALLED by compute_log_prob (operand pre-passes + the GEMM kernel);
+        # the kernel alone (prototype operands pre-staged) is an extra key
         from mgproto_b200 import _lib
         iso = ops.sigma_is_isotropic(sg)
         kname = "mgp_logprob_fwd [N,P] as called (math=%s): %s" % (
-            args.math, "tc_proto_prep + logprob_z_kernel (TMEM-resident patch tile, fused fp16 hi/lo split, TMA-store epilogue)"
+            args.math, "tc_proto_prep + logprob_z_kernel (patch operands in registers, fused fp16 hi/lo split, TMA-store epilogue)"
             if (iso and args.math == "auto") else "operand pre-passes + logprob kernel")
-        traffic = None
-        tp = os.path.join(ROOT, "profiles", "traffic.json")
-        if os.path.exists(tp):
-            traffic = json.load(open(tp)).get("logprob_dram_bytes_per_launch")
         roof = {"kernel": kname, "bound": "hbm", "achieved": abytes / t_op / 1e9,
-                "peak": peak, "unit": "GB/s", "frac": abytes / t_op / 1e9 / peak, "traffic": traffic,
-                "peak_source": how + " (MEASURED_PEAKS.json hbm_gbs, burst: op timed alone)",
+                "peak": peak, "unit": "GB/s", "frac": abytes / t_op / 1e9 / peak,
+                "peak_source": how if how != "measured" else "MEASURED_PEAKS.json hbm_gbs (burst: op timed alone)",
                 "us_per_launch": t_op * 1e6, "algorithmic_bytes": abytes,
                 "pairs_per_sec": N * P / t_op, "tensor_tflops_equiv": 4.0 * N * P * D / t_op / 1e12,
                 "note": "north-star kernel K-A (compute_log_prob / eval / push: log p materialised), the whole op as the "
-                        "API calls it, 6 x 25.7 MB inputs and 2 x 401 MB outputs rotating; the [N,P] TMA-store stream "
-                        "alone tops out at 5.1-5.5 TB/s on this part (profiles/r2_tma_store_bw.txt); the labelled training "
+                        "API calls it, 6 x 25.7 MB inputs and 2 x 401 MB outputs rotating; the labelled training "
                         "step runs the max/arg-max variant instead (roofline_step_logprob)"}
         if args.math != "fp32" and _lib.load().mgp_has_tensor_core_path():
             mode_full, mode_reuse = ("tc_iso", "tc_iso_reuse") if iso and D in (64, 128, 256) else ("tc", "tc_reuse")
@@ -595,7 +620,7 @@ def main():
         # the variant the labelled step runs: same GEMM, max/arg-max epilogue, no log p output -> tensor-bound
         pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))).get("bf16_tflops") if \
             os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else None
-        tpk, tsrc = (pk, "MEASURED_PEAKS.json bf16_tflops (burst)") if pk else (2250.0, "nominal dense bf16 (B200_PROFILING.md fallback)")
+        tpk, tsrc = (pk, "MEASURED_PEAKS.json bf16_tflops (burst)") if pk else (989.0, "H100 SXM data sheet, dense bf16")
         if args.math != "fp32" and _lib.load().mgp_has_tensor_core_path():
             w1 = [ops.logprob_top1(xs[i], mu, sg, B, HW, "tc", return_ws=True)[1] for i in range(6)]
             torch.cuda.synchronize()
@@ -616,7 +641,7 @@ def main():
                                         + 4.0 * B * c["K"] * D,
                 "kb_GBps": (4.0 * N * D + 8.0 * P * D + 8.0 * B * P * c["T"] + 4.0 * B * c["C"] * c["T"]
                             + 4.0 * B * c["K"] * D) / t_t1 / 1e9,
-                "frac_of_sustained_bf16": fl / t_t1 / 1e12 / 1431.0}
+                "frac_of_peak_bf16": fl / t_t1 / 1e12 / tpk}
             del w1
         # EM statistics kernel, same treatment (second kernel the north star names)
         order = torch.arange(c["C"], dtype=torch.int32, device=dev)
@@ -670,7 +695,7 @@ def main():
             torch.cuda.synchronize()
             t_ub = e0.elapsed_time(e1) / reps / 1e3
             extra["roofline_step_update_gmm"] = {
-                "kernel": "update_GMM = em_plan + em_tc_kernel (tcgen05; 200 active classes, %d EM loops; + one fill)" % Lp,
+                "kernel": "update_GMM = em_plan + em_tc_kernel (wgmma; 200 active classes, %d EM loops; + one fill)" % Lp,
                 "bound": "hbm", "achieved": ub / t_ug / 1e9, "peak": peak, "unit": "GB/s", "frac": ub / t_ug / 1e9 / peak,
                 "us_per_call": t_ug * 1e6, "algorithmic_bytes": ub,
                 "batch_active_classes": n_batch_active, "us_per_call_batch_active": t_ub * 1e6,

@@ -1,5 +1,5 @@
 /*
- * mgproto_b200 -- C ABI of the B200-native MGProto Gaussian-prototype hot path.
+ * mgproto_b200 -- C ABI of the CUDA-native (H100, sm_90a) MGProto Gaussian-prototype hot path.
  *
  * The reference (cwangrun/MGProto) has no FFI: its boundary is the Python surface of
  * model.MGProto (SURVEY.md section 8b).  Each entry point below replaces the reference code
@@ -35,7 +35,7 @@ extern "C" {
 
 /* math modes of the log-probability kernels */
 #define MGP_MATH_FP32 0     /* exact-form fp32 SIMT: sum_d ((x-mu)/(sigma+eps))^2          */
-#define MGP_MATH_TC 1       /* tcgen05 tensor cores, fp16 hi/lo split x3, fp32 accumulate  */
+#define MGP_MATH_TC 1       /* wgmma tensor cores, fp16 hi/lo split x3, fp32 accumulate    */
 #define MGP_MATH_AUTO 2     /* TC when the shape qualifies, else FP32                      */
 #define MGP_MATH_TC_REUSE 3 /* TC, operands (fp16 hi/lo split of x and of the prototypes) are
                                already staged in `ws` by the previous MGP_MATH_TC call with the
@@ -44,10 +44,10 @@ extern "C" {
                                prototype (true for every state the reference's loop reaches).
                                Extends the tensor-core path to D = 256; the kernel traps if the
                                assertion is false                                               */
-#define MGP_MATH_TC_ISO_REUSE 5 /* TC_ISO with the prototype-side operands already in ws (as TC_REUSE) */
+#define MGP_MATH_TC_ISO_REUSE 5 /* TC_ISO with the prototype-side operands already in ws; the patch side is rebuilt */
 /* OR-ed onto MGP_MATH_TC / _AUTO / _TC_ISO: the patch-side operands of `ws` (fp16 hi / lo split, |xhat|^2) were
  * written by mgp_normalize_fwd_stage for exactly this xhat_nd -- the tensor-core kernels that read staged patches skip
- * their own pre-pass (the TMEM-resident kernel reads fp32 xhat_nd and ignores the flag).  _ISO: staged with
+ * their own pre-pass (the register-resident kernel reads fp32 xhat_nd and ignores the flag).  _ISO: staged with
  * stage_aniso = 0, i.e. without the x^2 half an anisotropic sigma needs: the kernel faults if sigma turns out to be. */
 #define MGP_MATH_X_STAGED 0x100
 #define MGP_MATH_X_STAGED_ISO 0x200
@@ -63,14 +63,14 @@ extern "C" {
 
 int mgp_abi_version(void);
 const char* mgp_error_string(int code);
-/* 1 if the library was built with the sm_100a tcgen05 kernels */
+/* 1 if the library was built with the sm_90a tensor-core (wgmma) kernels */
 int mgp_has_tensor_core_path(void);
 /* Process-wide test / diagnosis switches (not part of the reference surface; the defaults are the product path).
  * key "tc_z": 1 (default; 0 if MGP_TC_NO_Z is set) = the [N,P] log-likelihood with isotropic sigma and D <= 128 takes the
- * TMEM-resident kernel (csrc/logprob_tcz.cu), 0 = always csrc/logprob_tc.cu;
+ * register-resident kernel (csrc/logprob_tcz.cu), 0 = always csrc/logprob_tc.cu;
  * key "em_tc": 1 (default; 0 if MGP_EM_NO_TC is set) = mgp_update_gmm may take the tensor-core kernel;
  * key "em_pipe": 1 (default; 0 if MGP_EM_NO_PIPE is set) = at D = 128 that kernel is the software-pipelined variant
- * (three row-tile buffers, one CTA per SM), 0 = one tile at a time (two CTAs per SM; what D = 256 always runs);
+ * (three row-tile buffers), 0 = one tile at a time (what D = 256 always runs);
  * key "em_fused": 1 (default; 0 if MGP_EM_UNFUSED is set in the environment) = mgp_update_gmm runs the single
  * cluster launch where the shape allows, 0 = always the multi-launch path (identical arithmetic, used by the
  * parity tests to cross-check the two).  Returns the previous value, or MGP_ERR_INVALID for an unknown key. */
@@ -109,10 +109,10 @@ int mgp_normalize_bwd(const float* g_xhat_nd, const float* xhat_nd, const float*
  * structure), mu/sigma [P,D]; `ws` is scratch of at least mgp_logprob_ws_bytes(B, HW, P, D, math)
  * bytes (the tensor-core path stages fp16 hi/lo operands there). */
 size_t mgp_logprob_ws_bytes(int B, int HW, int P, int D, int math);
-/* 1 if mgp_logprob_fwd with this layout / shape / math mode reads the fp32 patches itself (the TMEM-resident kernel,
- * csrc/logprob_tcz.cu), so that its workspace holds prototype-side operands only: a caller whose mu / sigma are
- * unchanged since the previous call with the same workspace may then pass MGP_MATH_TC_ISO_REUSE and skip the
- * prototype pre-pass (with the other tensor-core kernels *_REUSE also reuses the staged patches). */
+/* 1 if mgp_logprob_fwd with this layout / shape / math mode reads the fp32 patches itself (the register-resident
+ * kernel, csrc/logprob_tcz.cu), so that its workspace holds prototype-side operands only: a caller whose mu / sigma
+ * are unchanged since the previous call with the same workspace may then pass MGP_MATH_TC_ISO_REUSE and skip the
+ * prototype pre-pass (with the other tensor-core kernels _ISO_REUSE rebuilds the patch side, *_TC_REUSE reuses it). */
 int mgp_logprob_ws_is_prototype_only(int out_layout, int P, int D, int math);
 int mgp_logprob_fwd(const float* xhat_nd, const float* mu, const float* sigma, float eps,
                     float eps_log, float* out, int out_layout, int B, int HW, int P, int D,
@@ -265,7 +265,7 @@ int mgp_em_update(const float* stats, int n_split, int with_s2, int n_rows_total
 /* With the bank's shadow (shadow_h / shadow_l / shadow_xx, see mgp_bank_enqueue; may be NULL) and sigma_iso != 0 --
  * the caller's assertion that sigma is constant over d inside every prototype, which holds for every state the
  * reference's training loop reaches -- shapes K <= 16, D in {128, 256} run as ONE tensor-core launch after the planner
- * (csrc/em_tc.cu: both inner products as tcgen05 GEMMs on fp16 hi/lo splits).  The kernel re-checks sigma and sets
+ * (csrc/em_tc.cu: both inner products as wgmma GEMMs on fp16 hi/lo splits).  The kernel re-checks sigma and sets
  * status[0] = 1 (leaving that class untouched) if the assertion was wrong.  Otherwise: K <= 16, D in {64, 128}: one
  * fp32 cluster launch; any other shape: the launches listed above. */
 /* number of kernel launches mgp_update_gmm enqueues for this shape (2 = planner + single launch) */

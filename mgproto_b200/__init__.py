@@ -1,8 +1,8 @@
-"""mgproto_b200 -- B200-native implementation of MGProto's Gaussian-prototype hot path.
+"""mgproto_b200 -- CUDA-native (H100, sm_90a) implementation of MGProto's Gaussian-prototype hot path.
 
 Drop-in for the reference's ``model`` module on that path: ``construct_MGProto``, ``MGProto``
 (forward / push_forward / update_GMM / compute_log_prob / _e_step / ...), ``MemoryBank``.
-The compute lives in ``libmgproto_b200.so`` (hand-written sm_100a CUDA behind the C ABI in
+The compute lives in ``libmgproto_b200.so`` (hand-written sm_90a CUDA behind the C ABI in
 ``include/mgproto_b200.h``); importing the package requires the built library.
 """
 from . import _lib

@@ -84,7 +84,7 @@ def load():
         except Exception as e:  # noqa: BLE001
             raise MGProtoLibraryError(
                 "libmgproto_b200.so could not be loaded (%s) or rebuilt (%s). Run `python -m "
-                "mgproto_b200.build` (needs nvcc, sm_100a). There is no CPU fallback." % (first, e)) from e
+                "mgproto_b200.build` (needs nvcc, sm_90a). There is no CPU fallback." % (first, e)) from e
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)          # AttributeError if the symbol is missing: fail loudly
         fn.restype = res

@@ -18,7 +18,7 @@ extern "C" const char* mgp_error_string(int code) {
     switch (code) {
         case MGP_OK: return "ok";
         case MGP_ERR_INVALID: return "mgproto_b200: invalid argument (null pointer, non-positive size or misalignment)";
-        case MGP_ERR_UNSUPPORTED: return "mgproto_b200: shape not supported by the sm_100a kernels";
+        case MGP_ERR_UNSUPPORTED: return "mgproto_b200: shape not supported by the sm_90a kernels";
         case MGP_ERR_WORKSPACE: return "mgproto_b200: workspace too small";
         default: break;
     }
@@ -130,7 +130,8 @@ extern "C" int mgp_logprob_fwd(const float* xhat_nd, const float* mu, const floa
     if (math == MGP_MATH_TC || math == MGP_MATH_AUTO || math == MGP_MATH_TC_REUSE || iso_mode) {
         if (mgp_logprob_tc_supported(out_layout, B, HW, P, D, iso_mode))
             return mgp_logprob_tc_launch(xhat_nd, mu, sigma, eps, eps_log, out, out_layout, B, HW, P, D, ws, ws_bytes,
-                                         math == MGP_MATH_TC_REUSE || math == MGP_MATH_TC_ISO_REUSE, iso_mode, x_staged, st);
+                                         math == MGP_MATH_TC_REUSE ? 2 : (math == MGP_MATH_TC_ISO_REUSE ? 1 : 0), iso_mode,
+                                         x_staged, st);
         if (math != MGP_MATH_AUTO) return MGP_ERR_UNSUPPORTED;
     }
 #else

@@ -1,30 +1,31 @@
-// a10-a12 on the 5th-gen tensor cores: the whole update_GMM (ref model.py:277-301, :303-321, :367-401) of a single
+// a10-a12 on the Hopper tensor cores: the whole update_GMM (ref model.py:277-301, :303-321, :367-401) of a single
 // replica in ONE launch after em_plan, one CTA per class, for the shapes the shipped loop produces
 // (K <= 16 components, D = 128 or 256, sigma constant over d inside every component).
 //
 // Per class and EM loop the two inner products are GEMMs over the class's bank rows X [cap x D]:
 //     E-step     Q  [cap x K]  = X . A^T        A_k = -2 w_k mu_k          (q_nk = w_k (|x_n|^2 + |mu_k|^2) + Q_nk)
 //     statistics S1^T [D x K]  = X^T . R        R_nk = smoothed responsibility
-// They run as tcgen05.mma (kind::f16, fp32 accumulators in TMEM) on fp16 hi/lo splits -- hi*hi + lo*hi + hi*lo, 22
-// mantissa bits, the scheme of logprob_tc.cu -- of
+// They run as wgmma.mma_async (fp16 operands from shared memory, fp32 accumulators in registers) on fp16 hi/lo
+// splits -- hi*hi + lo*hi + hi*lo, 22 mantissa bits, the scheme of logprob_tc.cu -- of
 //   * the bank rows: a SHADOW of the fp32 bank kept in HBM as fp16 hi / lo of 256 x (written by the enqueue scatter,
 //     csrc/bank.cu), so a 128-row tile is four TMA boxes into 128B-swizzled shared memory with no conversion pass.
-//     The same tile serves both GEMMs: as the K-major A operand of the E-step (rows x d) and as the MN-major A operand
-//     of the statistics GEMM (d x rows) -- one copy, two descriptors;
+//     The same tile serves both GEMMs: as the K-major A operand of the E-step (rows x d) and as the MN-major
+//     (transposed) A operand of the statistics GEMM (d x rows) -- one copy, two descriptors;
 //   * the means operand A (rebuilt from the on-chip means after every Adam step) and the responsibilities R (written
-//     by the E-step epilogue), both split in registers and stored in the UMMA K-major SWIZZLE_128B layout.
+//     by the E-step epilogue), both split in registers and stored in the K-major SWIZZLE_128B layout.
 // Everything else (soft-max, S0, gradient, diversity term, Adam, pi momentum, the zero-gradient replay of the other
 // classes' steps) is fp32 SIMT on the class's state, which stays in registers / shared memory for the whole timeline
 // exactly as in em_fused_kernel (em.cu); thread d owns mean / moment elements (k, d) for all k.
 //
-// Per 128-row tile: TMA load (mbarrier) -> 2*D/16 E-step MMAs (hi rows 0-15 and lo rows 16-31 of the means share one
-// B block: one N = 32 and one N = 16 MMA per k-step) -> epilogue (tcgen05.ld, soft-max, R) -> 2*128/16 statistics MMAs
-// accumulating in TMEM across the tiles of the loop.  Two variants of the same kernel (template flag PIPE):
-//   * serial (D = 256; D = 128 when more classes are active than there are SMs): the phases of a tile run one after
-//     the other on one tile buffer, two CTAs per SM (D = 128) overlap each other's latencies;
-//   * pipelined (D = 128, one CTA per SM, classes in the planner's order): three tile buffers, two E-step accumulators
-//     and two R buffers; one thread issues TMA(t+1), the E-step MMAs of tile t and the statistics MMAs of tile t-1
-//     while warps 0-3 run the soft-max of tile t; idle warps apply the replay of inactive classes.
+// Warpgroup 0 (warps 0-3) runs the E-step of a 128-row tile (two m64 halves: m64n32 with the X hi rows against
+// [means hi ; means lo], m64n16 with the X lo rows against means hi) and its soft-max straight from the accumulator
+// fragments (the 16 components of a row sit in 4 lanes).  Warpgroup 1 (warps 4-7) runs the statistics GEMM of the
+// tile (D / 64 m64 blocks) and keeps S1 in its registers across the tiles of a loop; at the end of a loop it hands
+// S1 to the owners through shared memory.  Two variants of the same kernel (template flag PIPE):
+//   * serial (D = 256; D = 128 when more classes are active than there are SMs): one tile buffer, the statistics
+//     of a tile follow its soft-max;
+//   * pipelined (D = 128, one CTA per SM, classes in the planner's order): three tile buffers and two R buffers; the
+//     TMA load of tile t+1 and the statistics of tile t-1 run under the E-step and soft-max of tile t.
 // Both are enqueued and the planner's count of active classes decides on the device which one does the work.
 // HBM/L2 traffic: num_em_loop x (4 D + 4) bytes per bank row -- the algorithmic bytes of SURVEY 8(d) K-D.
 #include <cuda.h>
@@ -40,8 +41,8 @@ using namespace mgp_tc;
 
 constexpr float SX = 256.0f;      // shadow rows hold 256 x (fp16 hi + lo)
 constexpr float SR = 1024.0f;     // responsibilities are stored as 1024 r
-constexpr int TR = 128;           // bank rows per tile (UMMA M of the E-step, K extent of the statistics GEMM)
-constexpr int NK = 16;            // UMMA N: components padded to 16
+constexpr int TR = 128;           // bank rows per tile (M of the E-step, K extent of the statistics GEMM)
+constexpr int S1_STRIDE = 17;     // S1 hand-over [D][17] fp32 (padded against bank conflicts)
 
 struct EmTcParams {
     const float* xx;              // [C*cap] |x|^2 of the bank rows (shadow)
@@ -61,16 +62,13 @@ struct EmTcParams {
     float alpha, tau, omtau, lamda;
     int num_em_loop, C, K, cap, prof_class;
 };
-// stamp layout: prof[(tile_ctr * 8 + phase)]; phases: 0 TMA issued, 1 TMA landed, 2 E-step MMAs issued, 3 E-step done
-// (seen by thread 0), 4 epilogue done, 5 statistics MMAs issued, 6 loop tail entered, 7 loop tail done
+// stamp layout: prof[(tile_ctr * 8 + phase)]; phases: 0 TMA issued, 1 TMA landed (seen by thread 0), 4 soft-max done,
+// 5 statistics MMAs done, 6 loop tail entered, 7 loop tail done
 #define MGP_PROF(ctr, ph)                                                                          \
     do {                                                                                           \
         if (prm.prof && blockIdx.x == prm.prof_class && (ctr) < 64) prm.prof[(ctr) * 8 + (ph)] = clock64();  \
     } while (0)
 
-// PIPE (D = 128): three row-tile buffers, two E-step accumulators and two R buffers, so that the TMA load of tile t+1,
-// the E-step MMAs of tile t and the statistics MMAs of tile t-1 overlap the soft-max epilogue (one CTA per SM; the
-// planner's class list puts the active classes first).  !PIPE (D = 256: one 128 KB tile buffer fits): serial per tile.
 // Sum V = 32 R values per lane across the warp with V - R shuffles (a butterfly that halves the live set each round)
 // instead of 5 V: afterwards a[i], i < R, holds the warp total of entry R * lane + i.
 template <int V>
@@ -88,15 +86,14 @@ __device__ __forceinline__ void warp_multi_reduce(float (&a)[V], int lane) {
 }
 
 template <int D, int KT, bool PIPE>
-__global__ void __launch_bounds__(256, (D == 128 && !PIPE) ? 2 : 1)
+__global__ void __launch_bounds__(256, 1)
 em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_l, const EmTcParams prm) {
     constexpr int NCH = D / 64;                    // 64-element (128 B) chunks along d
     constexpr uint32_t CH_BYTES = TR * 128;        // one [128 rows x 64] fp16 block
     constexpr uint32_t X_BYTES = NCH * CH_BYTES;   // hi (lo follows)
-    constexpr int DB = D / 128;                    // 128-wide d blocks (statistics accumulators)
     constexpr int OWN = D;                         // threads owning mean/moment elements: thread d <-> (k, d) for all k
-    constexpr int TMEM_COLS = (D == 128 && !PIPE) ? 64 : 128;   // (PIPE: 2 x) 32 (E-step: hi.hi + lo.hi | hi.lo) + DB * 32 (statistics)
-    constexpr int ISSUER = 128;                    // the TMA / MMA issuing thread: lane 0 of warp 4 (warps 0-3 run the E-step epilogue)
+    constexpr int MB = D / 64;                     // m64 blocks of the statistics GEMM
+    constexpr int ISSUER = 128;                    // the TMA issuing thread: lane 0 of warp 4 (warps 0-3 run the E-step)
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
@@ -108,9 +105,10 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
     // rows 16-31 = lo, so ONE N = 32 MMA multiplies the row tile's hi half with both and an N = 16 MMA adds lo x hi
     const uint32_t o_a = NXBUF * 2 * X_BYTES;                             // [NCH][32][128 B]
     const uint32_t o_r = o_a + NCH * 4096;                                // NRBUF x [2 (64-row chunks)][32][128 B]
-    const uint32_t o_misc = o_r + NRBUF * 8192;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(bp + o_misc);            // !PIPE: tma, estep, stats | PIPE: xfull[3] xfree[3] efull[2] rfull[2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 10);
+    // S1 hand-over [D][S1_STRIDE]: its own region (!PIPE) or, PIPE, the tile buffer that is idle at the end of a loop
+    const uint32_t o_s1 = o_r + NRBUF * 8192;
+    const uint32_t o_misc = o_s1 + (PIPE ? 0u : (uint32_t)((D * S1_STRIDE * 4 + 15) & ~15));
+    uint64_t* bars = reinterpret_cast<uint64_t*>(bp + o_misc);            // !PIPE: tma, (unused), stats | PIPE: xfull[3] xfree[3] (unused)[2] rfull[2]
     float* s_e = reinterpret_cast<float*>(bars + 12);                     // [KT][KT]
     float* s_red = s_e + KT * KT;                                         // [8] + [8][16]
     float* s_w = s_red + 136;                                             // [16] w_k
@@ -124,7 +122,7 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
     constexpr bool MULTI = (NPAIR + KT) <= 64;                            // one transposing reduction (warp_multi_reduce)
     constexpr int PV = MULTI ? 32 * ((NPAIR + KT + 31) / 32) : NPAIR + KT;
     float* s_pair = s_misc + 8;                                           // [8 warps][PV]
-    const uint32_t bar_tma = smem_u32(bars), bar_e = bar_tma + 8, bar_s = bar_tma + 16;
+    const uint32_t bar_tma = smem_u32(bars), bar_s = bar_tma + 16;
 
     const int n_active = prm.sched[0], step0 = prm.sched[1];
     // PIPE: one CTA per SM, so the planner's class list (active classes first, in order) decides who starts first
@@ -282,21 +280,16 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
     if (warp == 6) replay_prepare(step0 + L * (ord + 1), L * (n_active - ord - 1), s_misc + 4);
 
     if (tid == 0) MGP_PROF(63, 1);
-    // ---- set-up: barriers, TMEM, sigma-derived constants, zeroed operand tiles
+    // ---- set-up: barriers, sigma-derived constants, zeroed operand tiles
     if (tid == 0) {
-        if (PIPE) {
-            for (int i = 0; i < 3; ++i) { mbar_init(bar_tma + 8u * i, 1); mbar_init(bar_tma + 8u * (3 + i), 1); }
-            for (int i = 0; i < 2; ++i) { mbar_init(bar_tma + 8u * (6 + i), 1); mbar_init(bar_tma + 8u * (8 + i), 4); }
+        if (PIPE) {                                  // xfree / rfull: one arrive per warp of the consuming warpgroup
+            for (int i = 0; i < 3; ++i) { mbar_init(bar_tma + 8u * i, 1); mbar_init(bar_tma + 8u * (3 + i), 4); }
+            for (int i = 0; i < 2; ++i) mbar_init(bar_tma + 8u * (8 + i), 4);
         } else {
             mbar_init(bar_tma, 1);
-            mbar_init(bar_e, 1);
-            mbar_init(bar_s, 1);
+            mbar_init(bar_s, 4);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
     }
     bool same = true;
     for (int i = tid; i < KD; i += 256) same = same && (sg_c[i] == sg_c[(i / D) * D]);
@@ -313,13 +306,9 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
         }
         s_w[tid] = w; s_ls[tid] = ls; s_pi[tid] = pi;
     }
-    tc_fence_before();
     const bool iso = __syncthreads_and(same ? 1 : 0) != 0;
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     if (!iso) {                                      // the host promised isotropic sigma: flag it, leave the class untouched
         if (tid == 0) atomicExch(prm.status, 1);
-        if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS));
         return;
     }
     if (tid == 0) MGP_PROF(63, 2);
@@ -330,13 +319,119 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
     const float n_rows = (float)cap;
     const float inv_den = 1.0f / (1.0f + (float)K * prm.alpha);
     const float div_scale = -4.0f * prm.lamda / ((float)K * (float)(K - 1));
-    // E-step: A = X (K-major), B = [means hi ; means lo] (K-major): N = 32 with X hi, N = 16 (hi only) with X lo
-    const uint32_t idesc_e32 = umma_idesc_f16(TR, 2 * NK, 0, 0), idesc_e16 = umma_idesc_f16(TR, NK, 0, 0);
-    // statistics: A = X^T (MN-major), B = [R hi ; R lo] (K-major)
-    const uint32_t idesc_s32 = umma_idesc_f16(128, 2 * NK, 1, 0), idesc_s16 = umma_idesc_f16(128, NK, 1, 0);
-    const uint32_t d_e = tmem_base;                                  // [128 rows x (16 hi.hi + lo.hi | 16 hi.lo)]
-    const uint32_t d_s = tmem_base + (PIPE ? 64 : 32);               // DB x [128 d x 32], same column split
     uint32_t tile_ctr = 0;                                           // tiles issued so far (mbarrier phases)
+    const int t4 = lane & 3, g8 = lane >> 2;                         // accumulator fragment coordinates (tc_ptx.cuh)
+    float s32[MB][16], s16[MB][8];                                   // warpgroup 1: S1 of the current loop
+#pragma unroll
+    for (int mb = 0; mb < MB; ++mb) {
+#pragma unroll
+        for (int j = 0; j < 16; ++j) s32[mb][j] = 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) s16[mb][j] = 0.f;
+    }
+
+    // E-step of one tile + soft-max + R (warpgroup 0).  E-step: A = X (K-major), B = [means hi ; means lo] (K-major):
+    // N = 32 with X hi, N = 16 (means hi only) with X lo; rows h * 64 + 16 warp + g8 + 8 rr of the tile, components
+    // k = 8 i + 2 t4 + j (columns k: hi.hi, 16 + k: hi.lo; the N = 16 accumulator: lo.hi).
+    // before_write() runs between the soft-max and the R stores (PIPE: wait until the R buffer is free)
+    auto estep_tile = [&](uint32_t xb, uint8_t* rbp, int t, float inv_a, float (&s0v)[4], auto&& before_write) {
+        float e32[2][16], e16[2][8];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+            for (int j = 0; j < 16; ++j) e32[h][j] = 0.f;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) e16[h][j] = 0.f;
+        }
+        wg_fence();
+#pragma unroll
+        for (int ks = 0; ks < D / 16; ++ks) {
+            const uint32_t xo = (uint32_t)(ks >> 2) * CH_BYTES + (uint32_t)(ks & 3) * 32u;
+            const uint64_t bd = gmma_desc(base + o_a + (uint32_t)(ks >> 2) * 4096u + (uint32_t)(ks & 3) * 32u);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {                            // rows 64 h .. 64 h + 63 of the tile: + 8 KiB
+                wg_mma_n32<0>(e32[h], gmma_desc(xb + o_xh + xo + (uint32_t)h * 8192u), bd, 1u);
+                wg_mma_n16<0>(e16[h], gmma_desc(xb + o_xl + xo + (uint32_t)h * 8192u), bd, 1u);
+            }
+        }
+        wg_commit();
+        wg_wait0();
+        float rr_v[2][2][4];
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr) {
+                const int row = t * TR + h * 64 + 16 * warp + g8 + 8 * rr;
+                const bool valid = row < cap;
+                const float xxv = valid ? __ldg(prm.xx + (size_t)c * cap + row) : 0.f;
+                float wl[4], mx = -INFINITY;
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+#pragma unroll
+                    for (int j = 0; j < 2; ++j) {
+                        const int k = 8 * i + 2 * t4 + j, idx = 4 * i + 2 * rr + j;
+                        const float acc = (e32[h][idx] + e16[h][idx]) + e32[h][idx + 8];
+                        const float qq = fmaf(s_w[k], xxv, acc * inv_a);
+                        wl[2 * i + j] = (k < K) ? s_cst[k] - 0.5f * qq : -INFINITY;   // lp + log(pi + eps)  (ref :316)
+                        mx = fmaxf(mx, wl[2 * i + j]);
+                    }
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                float se = 0.f;
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    const int k = 8 * (q >> 1) + 2 * t4 + (q & 1);
+                    wl[q] = (k < K) ? expf(wl[q] - mx) : 0.f;
+                    se += wl[q];
+                }
+                se += __shfl_xor_sync(0xffffffffu, se, 1);
+                se += __shfl_xor_sync(0xffffffffu, se, 2);
+                const float inv_se = 1.0f / se;
+#pragma unroll
+                for (int q = 0; q < 4; ++q) rr_v[h][rr][q] = valid ? fmaf(wl[q], inv_se, prm.alpha) * inv_den : 0.f;   // ref :380-383
+            }
+        before_write();
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int rr = 0; rr < 2; ++rr) {
+                    const int rt = h * 64 + 16 * warp + g8 + 8 * rr;     // row within the tile
+                    const uint32_t rbase = (uint32_t)(rt >> 6) * 4096u + (uint32_t)(rt & 7) * 2u;
+                    const int c16 = (rt & 63) >> 3;
+#pragma unroll
+                    for (int q = 0; q < 4; ++q) {
+                        const int k = 8 * (q >> 1) + 2 * t4 + (q & 1);
+                        if (k < K) {
+                            const float r = rr_v[h][rr][q];
+                            s0v[q] += r;
+                            const float rs = r * SR;
+                            const __half hh = __float2half_rn(rs);
+                            const uint32_t off = rbase + (uint32_t)k * 128u + (uint32_t)(((c16 ^ (k & 7)) & 7) << 4);
+                            *reinterpret_cast<__half*>(rbp + off) = hh;                                          // row k
+                            *reinterpret_cast<__half*>(rbp + off + 2048u) = __float2half_rn(rs - __half2float(hh));   // row 16 + k
+                        }
+                    }
+                }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // R stores -> visible to the MMA (async proxy)
+    };
+    // statistics of one tile (warpgroup 1): S1 += X^T . [R hi ; R lo] (m64n32, A = X hi MN-major) and X lo^T . R hi
+    // (m64n16), one m64 block per 64 d
+    auto stats_tile = [&](uint32_t xb, uint32_t rb, bool first) {
+        wg_fence();
+#pragma unroll
+        for (int ks = 0; ks < TR / 16; ++ks) {
+            const uint64_t bd = gmma_desc(rb + (uint32_t)(ks >> 2) * 4096u + (uint32_t)(ks & 3) * 32u);
+            const uint32_t acc = (first && ks == 0) ? 0u : 1u;
+#pragma unroll
+            for (int mb = 0; mb < MB; ++mb) {
+                const uint32_t xo = (uint32_t)mb * CH_BYTES + (uint32_t)ks * 2048u;   // 16 rows x 128 B
+                wg_mma_n32<1>(s32[mb], gmma_desc_mn(xb + o_xh + xo, CH_BYTES, 1024u), bd, acc);
+                wg_mma_n16<1>(s16[mb], gmma_desc_mn(xb + o_xl + xo, CH_BYTES, 1024u), bd, acc);
+            }
+        }
+        wg_commit();
+        wg_wait0();
+    };
 
     auto load_tile = [&](int t) {                                    // issuer only: one 128-row tile, hi + lo, into the X buffer
         mbar_expect_tx(bar_tma, 2 * X_BYTES);
@@ -432,19 +527,17 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // operand stores -> visible to the MMA (async proxy)
         __syncthreads();
 
-        float s0[KT];
-#pragma unroll
-        for (int k = 0; k < KT; ++k) s0[k] = 0.f;
+        float s0v[4] = {0.f, 0.f, 0.f, 0.f};                          // warpgroup 0: S0 of components 8 (q / 2) + 2 t4 + q % 2
         const float inv_a = 1.0f / (a_scale * SX);
+        uint32_t s1_base;                                             // the S1 hand-over of this loop
 
         if constexpr (PIPE) {
             // mbarriers: xfull[b] tile landed in buffer b | xfree[b] the statistics MMAs reading buffer b (and the R buffer
-            // they used) have retired | efull[e] E-step accumulator e complete | rfull[e] soft-max wrote R buffer e.
-            // Global tile counter g: row-tile buffer g % 3, accumulator / R buffer g & 1; every barrier completes exactly
-            // once per tile that uses its buffer, so its phase parity is (g / 3) & 1 resp. (g / 2) & 1.
+            // they used) have retired | rfull[e] soft-max wrote R buffer e.  Global tile counter g: row-tile buffer g % 3,
+            // R buffer g & 1; every barrier completes exactly once per tile that uses its buffer, so its phase parity is
+            // (g / 3) & 1 resp. (g / 2) & 1.
             auto XFULL = [&](uint32_t b) { return bar_tma + 8u * b; };
             auto XFREE = [&](uint32_t b) { return bar_tma + 8u * (3 + b); };
-            auto EFULL = [&](uint32_t e) { return bar_tma + 8u * (6 + e); };
             auto RFULL = [&](uint32_t e) { return bar_tma + 8u * (8 + e); };
             const uint32_t g0 = tile_ctr;
             auto load_tile_p = [&](int t, uint32_t g) {              // issuer: tile t of this class -> buffer g % 3
@@ -457,227 +550,108 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
                     tma_load_2d(base + b * 2 * X_BYTES + o_xh + ch * CH_BYTES, &map_h, ch * 64, row0, XFULL(b));
                     tma_load_2d(base + b * 2 * X_BYTES + o_xl + ch * CH_BYTES, &map_l, ch * 64, row0, XFULL(b));
                 }
+                MGP_PROF(g, 0);
             };
-            auto stats_mma = [&](int t, uint32_t g) {                // issuer: D_s += X(g)^T . [R_hi ; R_lo](g)
-                const uint32_t xb = base + (g % 3u) * 2 * X_BYTES, rb = base + o_r + (g & 1u) * 8192u;
-                mbar_wait(RFULL(g & 1u), (g >> 1) & 1u);
-                tc_fence_after();
-#pragma unroll
-                for (int ks = 0; ks < TR / 16; ++ks) {
-                    const uint32_t xo = (uint32_t)ks * 2048u;        // 16 rows x 128 B
-                    const uint64_t bd = umma_desc(rb + (uint32_t)(ks >> 2) * 4096u + (uint32_t)(ks & 3) * 32u);
-                    tc_mma_f16(d_s, umma_desc_mn(xb + o_xh + xo, CH_BYTES, 1024u), bd, idesc_s32, (t | ks) != 0);
-                    tc_mma_f16(d_s, umma_desc_mn(xb + o_xl + xo, CH_BYTES, 1024u), bd, idesc_s16, 1u);
+            if (warp >= 4) {
+                if (warp >= 5 && loop == 0) {                        // the absorbed inactive classes, before the first statistics
+                    for (int j = (int)blockIdx.x; j < ABSORB * n_active && n_active + j < prm.C; j += n_active)
+                        replay_inactive(prm.clist[n_active + j], 5, 3);
                 }
-                tc_commit(XFREE(g % 3u));
-                MGP_PROF(g, 5);
-            };
-            if (warp == ISSUER / 32) {
-                if (tid == ISSUER) {
-                    if (loop == 0) load_tile_p(0, g0);               // (later loops: prefetched under the previous loop's tail)
-                    for (int t = 0; t < ntiles; ++t) {
-                        const uint32_t g = g0 + t;
-                        MGP_PROF(g, 0);
-                        if (t + 1 < ntiles) load_tile_p(t + 1, g + 1);
-                        mbar_wait(XFULL(g % 3u), (g / 3u) & 1u);
-                        MGP_PROF(g, 1);
-                        tc_fence_after();
-                        const uint32_t xb = base + (g % 3u) * 2 * X_BYTES, de = d_e + (g & 1u) * 32u;
-#pragma unroll
-                        for (int ks = 0; ks < D / 16; ++ks) {
-                            const uint32_t xo = (uint32_t)(ks >> 2) * CH_BYTES + (uint32_t)(ks & 3) * 32u;
-                            const uint64_t bd = umma_desc(base + o_a + (uint32_t)(ks >> 2) * 4096u + (uint32_t)(ks & 3) * 32u);
-                            tc_mma_f16(de, umma_desc(xb + o_xh + xo), bd, idesc_e32, ks != 0);
-                            tc_mma_f16(de, umma_desc(xb + o_xl + xo), bd, idesc_e16, 1u);
-                        }
-                        tc_commit(EFULL(g & 1u));
-                        MGP_PROF(g, 2);
-                        if (t >= 1) stats_mma(t - 1, g - 1);
-                    }
-                    stats_mma(ntiles - 1, g0 + ntiles - 1);
-                    if (loop + 1 < L) load_tile_p(0, g0 + ntiles);   // the next loop's first tile, under this loop's tail
-                }
-                __syncwarp();
-            }
-            if (warp >= 5 && loop == 0) {                            // idle here: the absorbed inactive classes
-                for (int j = (int)blockIdx.x; j < ABSORB * n_active && n_active + j < prm.C; j += n_active)
-                    replay_inactive(prm.clist[n_active + j], 5, 3);
-            }
-            if (warp < 4) {
+                if (tid == ISSUER && loop == 0) load_tile_p(0, g0);  // (later loops: prefetched under the previous loop's tail)
                 for (int t = 0; t < ntiles; ++t) {
                     const uint32_t g = g0 + t;
-                    const int row = t * TR + tid;
-                    const bool valid = row < cap;
-                    const float xxv = valid ? __ldg(prm.xx + (size_t)c * cap + row) : 0.f;
-                    mbar_wait(EFULL(g & 1u), (g >> 1) & 1u);
-                    if (tid == 0) MGP_PROF(g, 3);
-                    tc_fence_after();
-                    uint32_t q[16], q1[16];
-                    const uint32_t de = d_e + (g & 1u) * 32u + ((uint32_t)(warp * 32) << 16);
-                    tmem_ld16(de, q);
-                    tmem_ld16(de + 16, q1);
-                    tmem_ld_wait();
-                    float wl[KT], mx = -INFINITY;
-#pragma unroll
-                    for (int k = 0; k < KT; ++k) {
-                        const float acc = __uint_as_float(q[k]) + __uint_as_float(q1[k]);
-                        const float qq = fmaf(s_w[k], xxv, acc * inv_a);
-                        wl[k] = (k < K) ? s_cst[k] - 0.5f * qq : -INFINITY;             // lp + log(pi + eps)  (ref :316)
-                        mx = fmaxf(mx, wl[k]);
-                    }
-                    float se = 0.f;
-#pragma unroll
-                    for (int k = 0; k < KT; ++k) {
-                        wl[k] = (k < K) ? expf(wl[k] - mx) : 0.f;
-                        se += wl[k];
-                    }
-                    const float inv_se = 1.0f / se;
-                    if (t >= 2) mbar_wait(XFREE((g - 2) % 3u), ((g - 2) / 3u) & 1u);   // the MMAs that read this R buffer have retired
-                    uint8_t* rbp = bp + o_r + (g & 1u) * 8192u;
-                    const uint32_t rbase = (uint32_t)(tid >> 6) * 4096u + (uint32_t)(tid & 7) * 2u;
-                    const int c16 = (tid & 63) >> 3;
-#pragma unroll
-                    for (int k = 0; k < KT; ++k)
-                        if (k < K) {
-                            const float r = valid ? fmaf(wl[k], inv_se, prm.alpha) * inv_den : 0.f;   // ref :380-383
-                            s0[k] += r;
-                            const float rs = r * SR;
-                            const __half h = __float2half_rn(rs);
-                            const uint32_t off = rbase + (uint32_t)k * 128u + (uint32_t)(((c16 ^ (k & 7)) & 7) << 4);
-                            *reinterpret_cast<__half*>(rbp + off) = h;                                         // row k
-                            *reinterpret_cast<__half*>(rbp + off + 2048u) = __float2half_rn(rs - __half2float(h));   // row 16 + k
-                        }
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                    tc_fence_before();
+                    if (tid == ISSUER && t + 1 < ntiles) load_tile_p(t + 1, g + 1);
+                    mbar_wait(XFULL(g % 3u), (g / 3u) & 1u);
+                    mbar_wait(RFULL(g & 1u), (g >> 1) & 1u);
+                    stats_tile(base + (g % 3u) * 2 * X_BYTES, base + o_r + (g & 1u) * 8192u, t == 0);
+                    if (tid == ISSUER) MGP_PROF(g, 5);
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(XFREE(g % 3u));
+                }
+                if (tid == ISSUER && loop + 1 < L) load_tile_p(0, g0 + ntiles);   // the next loop's first tile, under this loop's tail
+            } else {
+                for (int t = 0; t < ntiles; ++t) {
+                    const uint32_t g = g0 + t;
+                    mbar_wait(XFULL(g % 3u), (g / 3u) & 1u);
+                    if (tid == 0) MGP_PROF(g, 1);
+                    estep_tile(base + (g % 3u) * 2 * X_BYTES, bp + o_r + (g & 1u) * 8192u, t, inv_a, s0v, [&]() {
+                        if (t >= 2) mbar_wait(XFREE((g - 2) % 3u), ((g - 2) / 3u) & 1u);   // the MMAs that read this R buffer have retired
+                    });
                     __syncwarp();
                     if (tid == 0) MGP_PROF(g, 4);
                     if (lane == 0) mbar_arrive(RFULL(g & 1u));
                 }
+                const uint32_t gl = g0 + ntiles - 1;                 // the last statistics MMAs of this loop
+                mbar_wait(XFREE(gl % 3u), (gl / 3u) & 1u);
             }
             tile_ctr += (uint32_t)ntiles;
-            if (tid == 0) MGP_PROF(tile_ctr - 1, 6);
-            // ---- S0 over the class; the owners wait for the last statistics MMAs of this loop
-            if (warp < 4) {
-#pragma unroll
-                for (int k = 0; k < KT; ++k) {
-                    const float v = warp_sum(s0[k]);
-                    if (lane == 0) s_red[warp * 16 + k] = v;
-                }
-                const uint32_t gl = tile_ctr - 1;
-                mbar_wait(XFREE(gl % 3u), (gl / 3u) & 1u);
-                tc_fence_after();
-            }
-            __syncthreads();
+            s1_base = base + ((tile_ctr + 1u) % 3u) * 2 * X_BYTES;   // idle until the next loop's second tile
         } else {
         for (int t = 0; t < ntiles; ++t, ++tile_ctr) {
             const uint32_t par = tile_ctr & 1u;
             if (tid == ISSUER) {
-                MGP_PROF(tile_ctr, 0);
                 if (!(t == 0 && loop > 0)) {                                 // (a loop's first tile was prefetched by the previous loop)
                     if (tile_ctr > 0) mbar_wait(bar_s, (tile_ctr - 1) & 1u); // previous statistics MMAs have read X and R
                     load_tile(t);
+                    MGP_PROF(tile_ctr, 0);
                 }
-                mbar_wait(bar_tma, par);
-                MGP_PROF(tile_ctr, 1);
-                tc_fence_after();
-                // E-step: D_e[row, 0:32] = X_hi . [A_hi ; A_lo]^T (N = 32);  D_e[row, 0:16] += X_lo . A_hi^T (N = 16)
-#pragma unroll
-                for (int ks = 0; ks < D / 16; ++ks) {
-                    const uint32_t xo = (uint32_t)(ks >> 2) * CH_BYTES + (uint32_t)(ks & 3) * 32u;
-                    const uint64_t bd = umma_desc(base + o_a + (uint32_t)(ks >> 2) * 4096u + (uint32_t)(ks & 3) * 32u);
-                    tc_mma_f16(d_e, umma_desc(base + o_xh + xo), bd, idesc_e32, ks != 0);
-                    tc_mma_f16(d_e, umma_desc(base + o_xl + xo), bd, idesc_e16, 1u);      // lo.hi adds onto the hi.hi columns
-                }
-                tc_commit(bar_e);
-                MGP_PROF(tile_ctr, 2);
             }
             if (warp < 4) {
-                // ---- E-step epilogue: thread = bank row
-                const int row = t * TR + tid;
-                const bool valid = row < cap;
-                const float xxv = valid ? __ldg(prm.xx + (size_t)c * cap + row) : 0.f;
-                mbar_wait(bar_e, par);
-                if (tid == 0) MGP_PROF(tile_ctr, 3);
-                tc_fence_after();
-                uint32_t q[16], q1[16];
-                tmem_ld16(d_e + ((uint32_t)(warp * 32) << 16), q);
-                tmem_ld16(d_e + 16 + ((uint32_t)(warp * 32) << 16), q1);
-                tmem_ld_wait();
-                float wl[KT], mx = -INFINITY;
-#pragma unroll
-                for (int k = 0; k < KT; ++k) {
-                    const float acc = __uint_as_float(q[k]) + __uint_as_float(q1[k]);
-                    const float qq = fmaf(s_w[k], xxv, acc * inv_a);
-                    wl[k] = (k < K) ? s_cst[k] - 0.5f * qq : -INFINITY;                 // lp + log(pi + eps)  (ref :316)
-                    mx = fmaxf(mx, wl[k]);
-                }
-                float se = 0.f;
-#pragma unroll
-                for (int k = 0; k < KT; ++k) {
-                    wl[k] = (k < K) ? expf(wl[k] - mx) : 0.f;
-                    se += wl[k];
-                }
-                const float inv_se = 1.0f / se;
-                const uint32_t rbase = (uint32_t)(tid >> 6) * 4096u + (uint32_t)(tid & 7) * 2u;
-                const int c16 = (tid & 63) >> 3;
-#pragma unroll
-                for (int k = 0; k < KT; ++k)
-                    if (k < K) {
-                        const float r = valid ? fmaf(wl[k], inv_se, prm.alpha) * inv_den : 0.f;   // ref :380-383
-                        s0[k] += r;
-                        const float rs = r * SR;
-                        const __half h = __float2half_rn(rs);
-                        const uint32_t off = rbase + (uint32_t)k * 128u + (uint32_t)(((c16 ^ (k & 7)) & 7) << 4);
-                        *reinterpret_cast<__half*>(bp + o_r + off) = h;                                           // row k
-                        *reinterpret_cast<__half*>(bp + o_r + off + 2048u) = __float2half_rn(rs - __half2float(h));   // row 16 + k
-                    }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                tc_fence_before();
+                mbar_wait(bar_tma, par);
+                if (tid == 0) MGP_PROF(tile_ctr, 1);
+                estep_tile(base, bp + o_r, t, inv_a, s0v, []() {});
                 if (tid == 0) MGP_PROF(tile_ctr, 4);
             }
             __syncthreads();
-            if (tid == ISSUER) {
-                tc_fence_after();
-                // statistics: D_s[d, 0:32] += X_hi^T . [R_hi ; R_lo] (N = 32);  D_s[d, 0:16] += X_lo^T . R_hi (N = 16)
-#pragma unroll
-                for (int db = 0; db < DB; ++db) {
-#pragma unroll
-                    for (int ks = 0; ks < TR / 16; ++ks) {
-                        const uint32_t xo = (uint32_t)db * 2u * CH_BYTES + (uint32_t)ks * 2048u;   // 16 rows x 128 B
-                        const uint64_t bd = umma_desc(base + o_r + (uint32_t)(ks >> 2) * 4096u + (uint32_t)(ks & 3) * 32u);
-                        tc_mma_f16(d_s + db * 32, umma_desc_mn(base + o_xh + xo, CH_BYTES, 1024u), bd, idesc_s32, (t | ks) != 0);
-                        tc_mma_f16(d_s + db * 32, umma_desc_mn(base + o_xl + xo, CH_BYTES, 1024u), bd, idesc_s16, 1u);
-                    }
-                }
-                tc_commit(bar_s);
-                MGP_PROF(tile_ctr, 5);
+            if (warp >= 4) {
+                mbar_wait(bar_tma, par);                                     // (the tile is visible to this warpgroup's MMAs)
+                stats_tile(base, base + o_r, t == 0);
+                if (tid == ISSUER) MGP_PROF(tile_ctr, 5);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(bar_s);
             }
         }
-        if (tid == 0) MGP_PROF(tile_ctr - 1, 6);
         if (tid == ISSUER && loop + 1 < L) {          // the next loop starts on the same rows: fetch its first tile under the tail
             mbar_wait(bar_s, (tile_ctr - 1) & 1u);
             load_tile(0);
         }
-        // ---- S0 over the class, S1 from TMEM
-#pragma unroll
-        for (int k = 0; k < KT; ++k) {
-            float v = s0[k];
-            v = warp_sum(v);
-            if (lane == 0 && warp < 4) s_red[warp * 16 + k] = v;
-        }
         mbar_wait(bar_s, (tile_ctr - 1) & 1u);                        // all statistics MMAs of this loop have retired
-        tc_fence_after();
-        __syncthreads();
+        s1_base = base + o_s1;
         }   // !PIPE
-        if (tid < K) s_s0[tid] = (s_red[tid] + s_red[16 + tid]) + (s_red[32 + tid] + s_red[48 + tid]);
-        uint32_t sacc[16], sacc1[16];
-        if (own) {
-            const uint32_t ta = d_s + (uint32_t)(tid >> 7) * 32u + ((uint32_t)((warp & 3) * 32) << 16);
-            tmem_ld16(ta, sacc);
-            tmem_ld16(ta + 16, sacc1);
-            tmem_ld_wait();
+        if (tid == 0) MGP_PROF(tile_ctr - 1, 6);
+        // ---- S0 over the class (warpgroup 0: reduce over the 8 rows of a fragment column, then lanes 0-3 hold all 16)
+        if (warp < 4) {
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                float v = s0v[q];
+                v += __shfl_xor_sync(0xffffffffu, v, 4);
+                v += __shfl_xor_sync(0xffffffffu, v, 8);
+                v += __shfl_xor_sync(0xffffffffu, v, 16);
+                if (g8 == 0) s_red[warp * 16 + 8 * (q >> 1) + 2 * t4 + (q & 1)] = v;
+            }
         }
-        tc_fence_before();
+        // ---- S1 from warpgroup 1's registers to the owners: s1[d][k] = (hi.hi + lo.hi) + hi.lo
+        float* s_s1 = reinterpret_cast<float*>(bp + (s1_base - base));
+        if (warp >= 4) {
+#pragma unroll
+            for (int mb = 0; mb < MB; ++mb)
+#pragma unroll
+                for (int rr = 0; rr < 2; ++rr)
+#pragma unroll
+                    for (int q = 0; q < 4; ++q) {
+                        const int d = mb * 64 + 16 * (warp - 4) + g8 + 8 * rr, k = 8 * (q >> 1) + 2 * t4 + (q & 1);
+                        const int idx = 4 * (q >> 1) + 2 * rr + (q & 1);
+                        s_s1[d * S1_STRIDE + k] = (s32[mb][idx] + s16[mb][idx]) + s32[mb][idx + 8];
+                    }
+        }
+        __syncthreads();
+        if (tid < K) s_s0[tid] = (s_red[tid] + s_red[16 + tid]) + (s_red[32 + tid] + s_red[48 + tid]);
+        float sacc[KT];
+        if (own) {
+#pragma unroll
+            for (int k = 0; k < KT; ++k) sacc[k] = s_s1[tid * S1_STRIDE + k];
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // PIPE: the hand-over area is a TMA destination again
         __syncthreads();
         // ---- gradient + diversity + Adam on the owned elements (ref model.py:385-397; SURVEY KA6)
         if (own) {
@@ -689,7 +663,7 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
                 newp[k] = p_[k];
                 if (k < K) {
                     const float muv = p_[k];
-                    const float s1 = (__uint_as_float(sacc[k]) + __uint_as_float(sacc1[k])) * (1.0f / (SX * SR));
+                    const float s1 = sacc[k] * (1.0f / (SX * SR));
                     float g = -(s1 - muv * s_s0[k]) * s_w[k] / n_rows;
                     float esum = 0.f, emu = 0.f;
 #pragma unroll
@@ -719,18 +693,13 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
     if (tid == 0) MGP_PROF(63, 5);
     write_back();
     if (tid < K) prm.weight[(size_t)c * P + (size_t)c * K + tid] = s_pi[tid];
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS));
-    }
     if (tid == 0) MGP_PROF(63, 6);
 }
 
 template <int D>
 size_t em_tc_smem(int kt, bool pipe) {
     return 1024 + (pipe ? 3 : 1) * 2 * (size_t)(D / 64) * TR * 128 + (size_t)(D / 64) * 4096 + (pipe ? 2 : 1) * 8192 +
+           (pipe ? 0 : (size_t)((D * S1_STRIDE * 4 + 15) & ~15)) +
            ((size_t)kt * kt + 136 + 6 * 16 + 8 + 8 * (size_t)(32 * ((kt * (kt - 1) / 2 + kt + 31) / 32))) * 4 + 128;
 }
 

@@ -8,7 +8,7 @@
 // Register-tiled like an SGEMM (128x128 CTA tile, 8x8 per thread, K-step 16), but the
 // inner op is sub-mul-fma on the *difference* -- the same arithmetic form as the
 // reference, so the result carries no cancellation error.  3 issue slots per pair-dim:
-// this kernel is bound by the fp32 pipe (~1.1 ms at B=256, P=2000, D=128), not by HBM;
+// this kernel is bound by the fp32 pipe, not by HBM;
 // it is the exact path and the fallback for shapes the tensor-core kernel does not take.
 #include "mgp_common.cuh"
 

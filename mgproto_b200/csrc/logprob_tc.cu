@@ -1,4 +1,4 @@
-// a2/a16 on the 5th-gen tensor cores (MGP_MATH_TC): the squared Mahalanobis distance as a GEMM
+// a2/a16 on the Hopper tensor cores (MGP_MATH_TC): the squared Mahalanobis distance as a GEMM
 //
 //   q[n,p] = sum_d w_pd x_nd^2 - 2 sum_d (w mu)_pd x_nd + sum_d w_pd mu_pd^2 ,   w = 1/(sigma+eps)^2
 //          = [x^2 | x]_n . [w | -2 w mu]_p + c2_p                       (inner dim 2D, general diagonal)
@@ -7,20 +7,20 @@
 //   log p = e0_p + e1_p * acc[n,p] + e2_p * |x_n|^2
 //
 // Precision: operands are split into fp16 hi + lo (22 mantissa bits) and accumulated as
-// hi*hi + lo*hi + hi*lo in fp32 TMEM accumulators -- three kind::f16 passes instead of one TF32
+// hi*hi + lo*hi + hi*lo in fp32 register accumulators -- three fp16 wgmma passes instead of one TF32
 // pass at half rate; |error| on q ~1e-6, inside the 1e-4 bar on logits (a single bf16 or tf32
 // pass is not).  Power-of-two scalings keep the lo parts in fp16's normal range and are undone
 // exactly in the epilogue.
 //
-// Structure (one persistent CTA per SM, 12 warps):
-//   warp 0   TMA producer: prototype (A) K-blocks through an S-stage mbarrier ring
-//   warp 3   TMA producer of the x tile (B, 128 patches x Kg), resident per n-tile, double-buffered when
-//            sigma is isotropic so the next n-tile is prefetched under the current one's MMAs
-//   warp 1   one thread issues tcgen05.mma (M=128 prototypes x N=128 patches x K=16), 2 TMEM accumulators
-//   warp 2   TMEM allocator
-//   warps 4-11 epilogue: tcgen05.ld 32 lanes x 32 columns, affine fix-up, stores.  TMEM lane = prototype,
-//            column = patch, so for the [N,P] layout the 32 lanes of a warp write 32 consecutive floats
-//            of one output row -- fully coalesced straight from registers, no staging pass.
+// Structure (one persistent CTA per SM, 10 warps):
+//   warp 8   TMA producer: prototype (A) K-blocks through an S-stage mbarrier ring
+//   warp 9   TMA producer of the x tile (B, 128 patches x Kg), resident per n-tile, double-buffered when
+//            it fits so the next n-tile is prefetched under the current one's MMAs
+//   warps 0-7  two consumer warpgroups: warpgroup g issues wgmma.mma_async m64n32k16 for prototypes
+//            [64 g, 64 g + 64) of the 128-prototype tile x all patches of the x tile, then runs the epilogue:
+//            the accumulator goes through a shared-memory transpose so that a thread holds 32 patches of ONE
+//            prototype and the 32 lanes of a warp hold 32 consecutive prototypes (for the [N,P] layout: 32
+//            consecutive floats of one output row), affine fix-up, stores.
 // HBM traffic per launch: 4*N*P (output) + 8*N*Kg (fp16 hi/lo operand written by the prep pass and
 // read once) + 4*N*D (x) -- the output dominates; the kernel is bound by the HBM write stream.
 #include <cuda.h>
@@ -36,17 +36,14 @@ constexpr int LAYOUT_NP_TMA = 3; // internal: [N,P] output written by TMA bulk t
 constexpr int LAYOUT_BPHW_TMA = 4;   // internal: [B,P,HW] log p through a 3-D tensor map (boxes clipped at image ends)
 constexpr int LAYOUT_NEGP_TMA = 5;   // internal: [B,P,HW] -exp(log p), same
 constexpr int LAYOUT_TOP1 = 6;       // internal: no log p output at all -- per (image, prototype) max / arg-max (MGP_OUT_TOP1_BP)
-constexpr int STAGING_BYTES = 8 * 32 * 32 * 4;   // one [32 patches x 32 prototypes] fp32 block per epilogue warp
-constexpr int PT = 128;          // prototypes per tile (UMMA M)
+constexpr int STAGING_BYTES = 8 * 32 * 32 * 4;   // one [32 x 32] fp32 block per consumer warp (transpose, TMA stores)
+constexpr int PT = 128;          // prototypes per tile (two warpgroups x 64)
 constexpr int KB = 64;           // K elements per smem block (128 B rows, SWIZZLE_128B)
 constexpr int SUB_BYTES = 128 * KB * 2;   // one [128 x 64] fp16 block = 16 KiB
 constexpr float X_SCALE = 256.0f;
 
 // ------------------------------------------------------------------------------------------ PTX (tc_ptx.cuh)
 using namespace mgp_tc;
-
-// kind::f16 instruction descriptor of the [PT prototypes x n_tile patches] tile, both operands K-major
-__device__ __forceinline__ uint32_t make_idesc(int n_tile) { return umma_idesc_f16(PT, n_tile); }
 
 // ------------------------------------------------------------------------------------------ prep
 // Prototype side: Bh/Bl [P, 2D] fp16 = split of scale_p * [ w | -2 w mu ]; e0,e1,e2 [P]; noniso flag.
@@ -152,11 +149,11 @@ struct TcParams {
                            // adjacent prototype tiles, so each output row receives team*512 contiguous bytes at once
     uint32_t smem_bytes;   // dynamic shared memory of the launch
     int x_no_sq;           // the staged patch operands lack the x^2 half (isotropic sigma asserted by the producer)
-    int debug;   // ablation switches for profiling (MGP_TC_DEBUG): 1 no global stores, 2 no TMEM loads, 4 no MMAs,
+    int debug;   // ablation switches for profiling (MGP_TC_DEBUG): 1 no global stores, 4 no MMAs,
                  // 8 no epilogue work, 16 no prototype TMA loads
 };
 
-constexpr int TC_THREADS = 384;   // warps: 0 proto TMA, 1 MMA, 2 TMEM alloc, 3 x-tile TMA, 4..11 epilogue
+constexpr int TC_THREADS = 320;   // warps: 0-7 two consumer warpgroups (MMA + epilogue), 8 proto TMA, 9 x-tile TMA
 
 template <int LAYOUT>
 __device__ __forceinline__ void epilogue_chunk(const uint32_t (&r)[32], const float* __restrict__ s_sn_c, float c0,
@@ -314,6 +311,8 @@ logprob_tc_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_const
                   const __grid_constant__ CUtensorMap map_out, const TcParams prm) {
     constexpr bool TMA_ST = (LAYOUT == LAYOUT_NP_TMA || LAYOUT == LAYOUT_BPHW_TMA || LAYOUT == LAYOUT_NEGP_TMA);
     constexpr bool BPHW_TMA = (LAYOUT == LAYOUT_BPHW_TMA || LAYOUT == LAYOUT_NEGP_TMA);
+    // image tiles (up to 256 patches = 8 chunks) exist only for these layouts; 128-patch tiles have 4 chunks
+    constexpr int NCH = (BPHW_TMA || LAYOUT == LAYOUT_TOP1) ? 8 : 4;
     // the layout used by the non-TMA fallback of the same instantiation (anisotropic sigma: see `img` below)
     constexpr int STG_LAYOUT = (LAYOUT == LAYOUT_BPHW_TMA) ? MGP_OUT_LOGP_BPHW
                                : (LAYOUT == LAYOUT_NEGP_TMA) ? MGP_OUT_NEGP_BPHW : LAYOUT;
@@ -326,61 +325,43 @@ logprob_tc_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_const
     if (gen && (prm.D > 128 || prm.x_no_sq)) __trap();            // isotropic sigma was promised (MGP_MATH_TC_ISO / staging): fail loudly
     const int nkb = (gen ? 2 * prm.D : prm.D) / KB;               // K blocks per tile
     const int kcol0 = gen ? 0 : prm.D;                            // isotropic: only the [x] / [-2 w mu] half
-    // [B,P,HW] through TMA: one x tile = one image (nti = round_up(HW,32) columns, UMMA N = nti) so that no
-    // 32-column chunk crosses an image end.  The wider tile only fits when sigma is isotropic (K = D);
-    // otherwise this instantiation falls back to 128-patch tiles and register stores.
+    // [B,P,HW] through TMA: one x tile = one image (nti = round_up(HW,32) patches) so that no 32-column chunk
+    // crosses an image end.  The wider tile only fits when sigma is isotropic (K = D); otherwise this
+    // instantiation falls back to 128-patch tiles and register stores.
     const bool img = (BPHW_TMA || (LAYOUT == LAYOUT_TOP1 && prm.xbox == 32)) && !gen;
-    const int NT = img ? prm.nti : 128;                           // patches per tile = UMMA N
+    const int NT = img ? prm.nti : 128;                           // patches per tile
+    const int nch = NT / 32;                                      // 32-patch MMA chunks (m64n32k16 each)
     const int row_step = img ? prm.HW : 128;                      // first patch row of x tile nt = nt * row_step
-    // image tiles: the x tile holds nti = round_up(HW, 32) rows (whole 32-row TMA boxes), the MMA only spans
-    // round_up(HW, 16) of them (HW = 196: N = 208 instead of 224); the columns beyond are never read (masked / clipped)
-    const uint32_t idesc = make_idesc(img ? ((prm.HW + 15) & ~15) : NT);
     const int n_ptiles = prm.n_ptiles, n_ntiles = img ? prm.B : prm.n_ntiles;
     const uint32_t xsub = (uint32_t)NT * KB * 2;                  // one [NT x 64] fp16 block of the x tile
 
-    // carve-up: nbuf x tiles | S stages of (proto hi, proto lo) | [TMA-store staging] | barriers + sn tile
+    // carve-up: nbuf x tiles | S stages of (proto hi, proto lo) | staging (accumulator transpose + TMA stores) | barriers + sn tile
     const uint32_t x_bytes = (uint32_t)(2 * nkb) * xsub;          // hi blocks then lo blocks
-    const uint32_t tile_budget = prm.smem_bytes - 1024u - 2048u - (TMA_ST ? (uint32_t)STAGING_BYTES : 0u);
+    const uint32_t tile_budget = prm.smem_bytes - 1024u - 2048u - (uint32_t)STAGING_BYTES;
     const int nbuf = (2 * x_bytes + 2 * 2 * SUB_BYTES <= tile_budget) ? 2 : 1;   // double-buffer x when it fits
     int S = (int)((tile_budget - nbuf * x_bytes) / (2 * SUB_BYTES));
     if (S > 6) S = 6;
     const uint32_t x_base = base;
     const uint32_t st_base = x_base + nbuf * x_bytes;
     const uint32_t stg_base = st_base + (uint32_t)S * 2 * SUB_BYTES;
-    const uint32_t misc = stg_base + (TMA_ST ? (uint32_t)STAGING_BYTES : 0u);
+    const uint32_t misc = stg_base + (uint32_t)STAGING_BYTES;
     float* staging = reinterpret_cast<float*>(base_ptr + (stg_base - base));
     uint8_t* misc_ptr = base_ptr + (misc - base);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(misc_ptr);       // full[6] empty[6] xfull[2] xempty[2] tfull[2] tempty[2]
-    const uint32_t bar0 = misc;
+    const uint32_t bar0 = misc;                                   // full[6] empty[6] xfull[2] xempty[2]
     auto FULL = [&](int i) { return bar0 + 8u * i; };
     auto EMPTY = [&](int i) { return bar0 + 8u * (6 + i); };
     auto XFULL = [&](int i) { return bar0 + 8u * (12 + i); };
     auto XEMPTY = [&](int i) { return bar0 + 8u * (14 + i); };
-    auto TFULL = [&](int i) { return bar0 + 8u * (16 + i); };
-    auto TEMPTY = [&](int i) { return bar0 + 8u * (18 + i); };
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 20);
-    float* s_sn = reinterpret_cast<float*>(bars + 22);            // [256] |x|^2 of the current x tile, 16 B aligned
+    float* s_sn = reinterpret_cast<float*>(misc_ptr + 8 * 16);    // [256] |x|^2 of the current x tile, 16 B aligned
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < 6; ++i) { mbar_init(FULL(i), 1); mbar_init(EMPTY(i), 1); }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(XFULL(i), 1);
-            mbar_init(XEMPTY(i), 1);
-            mbar_init(TFULL(i), 1);
-            mbar_init(TEMPTY(i), 8);
-        }
+        for (int i = 0; i < 6; ++i) { mbar_init(FULL(i), 1); mbar_init(EMPTY(i), 8); }   // empty: one arrive per consumer warp
+        for (int i = 0; i < 2; ++i) { mbar_init(XFULL(i), 1); mbar_init(XEMPTY(i), 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     // schedule: team t = blockIdx / team handles x tiles t, t + n_teams, ...; member k of the team takes the
     // prototype tiles k, k + team, ... of each of them
@@ -390,7 +371,7 @@ logprob_tc_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_const
 
     if (!has_work) {
         // nothing to do for this CTA (tiny problems)
-    } else if (warp == 3 && lane == 0) {
+    } else if (warp == 9 && lane == 0) {
         // =========================== x-tile TMA producer (next x tile prefetched when double-buffered) ===========
         int c = 0;
         for (int nt = team; nt < n_ntiles; nt += n_teams, ++c) {
@@ -405,7 +386,7 @@ logprob_tc_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_const
                     tma_load_2d(xb + (uint32_t)(nkb + kb) * xsub + ro, &map_xl, kcol0 + kb * KB, nt * row_step + r, XFULL(buf));
                 }
         }
-    } else if (warp == 0 && lane == 0) {
+    } else if (warp == 8 && lane == 0) {
         // =========================== prototype TMA producer ===========================
         int stage = 0;
         uint32_t phase = 0;
@@ -425,127 +406,122 @@ logprob_tc_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_const
                 }
             }
         }
-    } else if (warp == 1 && lane == 0) {
-        // =========================== MMA issuer ===========================
-        int stage = 0, acc = 0, c = 0;
-        uint32_t phase = 0, acc_par = 0;
+    } else if (warp < 8) {
+        // =========================== consumers: MMA + epilogue ===========================
+        // warpgroup wg multiplies prototype rows [64 wg, 64 wg + 64) of the tile with all NT patches (nch m64n32 MMAs
+        // per K step, hi*hi + lo*hi + hi*lo into the same fp32 registers), then drains the accumulator 64 patches
+        // at a time through its transpose block: thread u of the warpgroup takes prototype row u % 64, chunk u / 64
+        // of the pass -- 32 consecutive prototypes per warp, 32 patches per thread, as epilogue_chunk expects.
+        // The transpose block [64 prototypes][64 patches] fp32 is the warpgroup's four TMA-store blocks; float column c
+        // of row r sits at c ^ 4 (r & 7) (conflict-free float4 reads).
+        const int wg = warp >> 2, wq = warp & 3, u = threadIdx.x & 127;
+        const int trow = u & 63, tsub = u >> 6;
+        float* tp = staging + wg * 4096;
+        float* stg = staging + warp * 1024;                       // this warp's 4 KiB TMA-store block
+        const uint32_t wg_bar = 2 + wg;
+        auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(wg_bar) : "memory"); };
+        int stage = 0, c = 0;
+        uint32_t phase = 0;
         for (int nt = team; nt < n_ntiles; nt += n_teams, ++c) {
             const int buf = c % nbuf;
-            mbar_wait(XFULL(buf), (uint32_t)((c / nbuf) & 1));
-            const uint32_t xb = x_base + (uint32_t)buf * x_bytes;
-            for (int pt = k0; pt < n_ptiles; pt += TS) {
-                mbar_wait(TEMPTY(acc), acc_par ^ 1u);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * NT);
-                for (int kb = 0; kb < nkb; ++kb) {
-                    mbar_wait(FULL(stage), phase);
-                    tc_fence_after();
-                    const uint32_t ph = st_base + (uint32_t)stage * 2 * SUB_BYTES, pl = ph + SUB_BYTES;
-                    const uint32_t xh = xb + (uint32_t)kb * xsub, xl = xb + (uint32_t)(nkb + kb) * xsub;
-#pragma unroll
-                    for (int k = 0; k < KB / 16; ++k) {
-                        if (prm.debug & 4) continue;
-                        const uint32_t off = (uint32_t)k * 32u;   // 16 fp16 = 32 B inside the 128 B swizzle row
-                        const uint64_t a_h = umma_desc(ph + off), a_l = umma_desc(pl + off);
-                        const uint64_t b_h = umma_desc(xh + off), b_l = umma_desc(xl + off);
-                        tc_mma_f16(d_tmem, a_h, b_h, idesc, (kb | k) != 0);
-                        tc_mma_f16(d_tmem, a_l, b_h, idesc, 1u);
-                        tc_mma_f16(d_tmem, a_h, b_l, idesc, 1u);
-                    }
-                    tc_commit(EMPTY(stage));                      // frees the stage when these MMAs retire
-                    if (++stage == S) { stage = 0; phase ^= 1u; }
-                }
-                tc_commit(TFULL(acc));                            // accumulator ready for the epilogue
-                acc ^= 1;
-                if (acc == 0) acc_par ^= 1u;
-            }
-            tc_commit(XEMPTY(buf));                               // x buffer may be refilled
-        }
-    } else if (warp >= 4) {
-        // =========================== epilogue ===========================
-        // 8 warps drain each accumulator together: warp = (TMEM lane quarter q, column half h)
-        const int e = warp - 4;
-        const int q = e & 3, h = e >> 2;
-        const int et = q * 32 + lane;                             // prototype row within the tile (TMEM lane)
-        const int nch_all = NT / 32;                              // 4 chunks (NT = 128) or up to 8 (image tiles)
-        const int ch0 = h ? (nch_all + 1) / 2 : 0, ch1 = h ? nch_all : (nch_all + 1) / 2;   // this warp's chunks
-        float* stg = staging + e * 1024;                          // this warp's 4 KiB TMA-store block
-        int acc = 0, c = 0;
-        uint32_t acc_par = 0;
-        const bool skip_epi = (prm.debug & 8) != 0;
-        for (int nt = team; nt < n_ntiles; nt += n_teams, ++c) {
             const int row0 = nt * row_step;
             asm volatile("bar.sync 1, 256;" ::: "memory");        // readers of the previous x tile's norms are done
-            for (int i = e * 32 + lane; i < NT; i += 256) {
+            for (int i = threadIdx.x; i < NT; i += 256) {
                 const int n = row0 + i;
                 s_sn[i] = (n < prm.N) ? prm.sn[n] : 0.f;
             }
             asm volatile("bar.sync 1, 256;" ::: "memory");
+            mbar_wait(XFULL(buf), (uint32_t)((c / nbuf) & 1));
+            const uint32_t xb = x_base + (uint32_t)buf * x_bytes;
             for (int pt = k0; pt < n_ptiles; pt += TS) {
-                const int p = pt * PT + et;
+                float acc[NCH][16];
+#pragma unroll
+                for (int ch = 0; ch < NCH; ++ch)
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) acc[ch][j] = 0.f;
+                for (int kb = 0; kb < nkb; ++kb) {
+                    mbar_wait(FULL(stage), phase);
+                    const uint32_t ph = st_base + (uint32_t)stage * 2 * SUB_BYTES + (uint32_t)wg * 64u * 128u, pl = ph + SUB_BYTES;
+                    const uint32_t xh = xb + (uint32_t)kb * xsub, xl = xb + (uint32_t)(nkb + kb) * xsub;
+                    if (!(prm.debug & 4)) {
+                        wg_fence();
+#pragma unroll
+                        for (int k = 0; k < KB / 16; ++k) {
+                            const uint32_t off = (uint32_t)k * 32u;   // 16 fp16 = 32 B inside the 128 B swizzle row
+                            const uint64_t a_h = gmma_desc(ph + off), a_l = gmma_desc(pl + off);
+#pragma unroll
+                            for (int ch = 0; ch < NCH; ++ch) {
+                                if (ch < nch) {
+                                    const uint32_t xo = (uint32_t)ch * 32u * 128u + off;   // 32 patch rows = 4 KiB
+                                    const uint64_t b_h = gmma_desc(xh + xo), b_l = gmma_desc(xl + xo);
+                                    wg_mma_n32<0>(acc[ch], a_h, b_h, 1u);
+                                    wg_mma_n32<0>(acc[ch], a_l, b_h, 1u);
+                                    wg_mma_n32<0>(acc[ch], a_h, b_l, 1u);
+                                }
+                            }
+                        }
+                        wg_commit();
+                        wg_wait0();
+                    }
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(EMPTY(stage));    // this warp no longer reads the stage
+                    if (++stage == S) { stage = 0; phase ^= 1u; }
+                }
+                if (pt + TS >= n_ptiles) {                        // last prototype tile of this x tile: release the buffer
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(XEMPTY(buf));
+                }
+                if (prm.debug & 8) continue;
+                const int p = pt * PT + wg * 64 + trow;
                 const bool pok = p < prm.P;
                 const float c0 = pok ? __ldg(prm.e0 + p) : 0.f;
                 const float c1 = pok ? __ldg(prm.e1 + p) : 0.f;
                 const float c2 = (pok && !gen) ? __ldg(prm.e2 + p) : 0.f;
-                mbar_wait(TFULL(acc), acc_par);
-                tc_fence_after();
-                if (!skip_epi) {
-                    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * NT);
-                    float run_v = -INFINITY;                      // LAYOUT_TOP1, image tiles: best of this warp's chunks
-                    int run_i = -1;
-#pragma unroll 1
-                    for (int ch = ch0; ch < ch1; ch += 2) {
-                        uint32_t r0[32], r1[32];
-                        const bool two = ch + 1 < ch1;
-                        if (!(prm.debug & 2)) {
-                            tmem_ld32(taddr + (uint32_t)ch * 32u, r0);
-                            if (two) tmem_ld32(taddr + (uint32_t)(ch + 1) * 32u, r1);
-                        } else {
+                float run_v = -INFINITY;                          // LAYOUT_TOP1, image tiles: best of this thread's chunks
+                int run_i = -1;
 #pragma unroll
-                            for (int j = 0; j < 32; ++j) { r0[j] = 0u; r1[j] = 0u; }
+                for (int pass = 0; pass < NCH / 2; ++pass) {
+                    if (2 * pass >= nch) break;
+                    // the TMA engine has read this warp's previous store block, and every reader of the previous pass is done
+                    if (TMA_ST && lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+                    wg_sync();
+                    const int r = 16 * wq + (lane >> 2), sw = 4 * (r & 7);    // (r + 8) & 7 == r & 7
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) {                 // n8 block i of this pass -> chunk 2 pass + i / 4
+                        const int ch = 2 * pass + (i >> 2), ib = i & 3;
+                        if (ch < nch) {
+                            const int col = (8 * i + 2 * (lane & 3)) ^ sw;
+                            *reinterpret_cast<float2*>(tp + r * 64 + col) = make_float2(acc[ch][4 * ib], acc[ch][4 * ib + 1]);
+                            *reinterpret_cast<float2*>(tp + (r + 8) * 64 + col) = make_float2(acc[ch][4 * ib + 2], acc[ch][4 * ib + 3]);
                         }
-                        tmem_ld_wait();
-                        if (ch + 2 >= ch1) {                      // accumulator slice is in registers: release it
-                            tc_fence_before();
-                            __syncwarp();
-                            if (lane == 0) mbar_arrive(TEMPTY(acc));
+                    }
+                    wg_sync();
+                    const int ch = 2 * pass + tsub;
+                    uint32_t rv[32];
+                    if (ch < nch) {
+                        const float4* src = reinterpret_cast<const float4*>(tp + trow * 64 + 32 * tsub);
+#pragma unroll
+                        for (int q = 0; q < 8; ++q) {
+                            const float4 f = src[q ^ (trow & 7)];
+                            rv[4 * q] = __float_as_uint(f.x); rv[4 * q + 1] = __float_as_uint(f.y);
+                            rv[4 * q + 2] = __float_as_uint(f.z); rv[4 * q + 3] = __float_as_uint(f.w);
                         }
-                        if (!BPHW_TMA || img) {
-                            epilogue_chunk<LAYOUT>(r0, s_sn + ch * 32, c0, c1, c2, row0 + ch * 32, p, pok, prm, stg, &map_out,
+                    }
+                    if (TMA_ST) wg_sync();                        // the store blocks are free for epilogue_chunk
+                    if (ch < nch) {
+                        if (!BPHW_TMA || img)
+                            epilogue_chunk<LAYOUT>(rv, s_sn + ch * 32, c0, c1, c2, row0 + ch * 32, p, pok, prm, stg, &map_out,
                                                    nt, ch * 32, img, &run_v, &run_i);
-                            if (two)
-                                epilogue_chunk<LAYOUT>(r1, s_sn + (ch + 1) * 32, c0, c1, c2, row0 + (ch + 1) * 32, p, pok, prm,
-                                                       stg, &map_out, nt, (ch + 1) * 32, img, &run_v, &run_i);
-                        } else {
-                            epilogue_chunk<STG_LAYOUT>(r0, s_sn + ch * 32, c0, c1, c2, row0 + ch * 32, p, pok, prm);
-                            if (two)
-                                epilogue_chunk<STG_LAYOUT>(r1, s_sn + (ch + 1) * 32, c0, c1, c2, row0 + (ch + 1) * 32, p, pok, prm);
-                        }
+                        else
+                            epilogue_chunk<STG_LAYOUT>(rv, s_sn + ch * 32, c0, c1, c2, row0 + ch * 32, p, pok, prm);
                     }
-                    if (LAYOUT == LAYOUT_TOP1 && img && pok && run_i >= 0 && !(prm.debug & 1))
-                        atomicMax(reinterpret_cast<unsigned long long*>(prm.out) + (size_t)nt * prm.P + p,
-                                  top1_pack(run_v, run_i));
-                    if (ch0 >= ch1) {                             // (never for NT >= 64; keeps the barrier count right)
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(TEMPTY(acc));
-                    }
-                } else {
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(TEMPTY(acc));
                 }
-                acc ^= 1;
-                if (acc == 0) acc_par ^= 1u;
+                if (LAYOUT == LAYOUT_TOP1 && img && pok && run_i >= 0 && !(prm.debug & 1))
+                    atomicMax(reinterpret_cast<unsigned long long*>(prm.out) + (size_t)nt * prm.P + p,
+                              top1_pack(run_v, run_i));
             }
         }
         if (TMA_ST && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // stores landed
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
     }
 }
 
@@ -604,7 +580,7 @@ WsLayout ws_layout(long long N, int P, int D) {
 
 }  // namespace
 
-// logprob_tcz.cu: [N,P] output, isotropic sigma, D <= 128: patch tile resident in TMEM, x split fused
+// logprob_tcz.cu: [N,P] output, isotropic sigma, D <= 128: patch operands resident in registers, x split fused
 bool mgp_logprob_tcz_supported(int P, int D);
 int mgp_logprob_tcz_launch(const float* xhat, const void* bh, const void* bl, const float* e0, const float* e1,
                            const float* e2, const int* noniso, float* out, long long N, int P, int D, cudaStream_t st);
@@ -649,16 +625,17 @@ int mgp_logprob_tc_launch(const float* xhat, const float* mu, const float* sigma
     float* sn = reinterpret_cast<float*>(wsb + w.sn);
     int* flag = reinterpret_cast<int*>(wsb + w.flag);
 
-    // [N,P] with isotropic sigma (asserted by the caller) and D <= 128: the TMEM-resident kernel reads fp32 x itself
+    // [N,P] with isotropic sigma (asserted by the caller) and D <= 128: the register-resident kernel reads fp32 x itself
     const bool use_z = (layout == MGP_OUT_LOGP_NP) && assume_iso && mgp_opt_tc_z() && mgp_logprob_tcz_supported(P, D);
-    if (!reuse_operands) {
+    // reuse_operands: 0 = prepare both operand sides, 1 = the prototype side is already in ws, 2 = both sides are
+    if (reuse_operands == 0) {
         MGP_CUDA(cudaMemsetAsync(flag, 0, 4, st));
         tc_proto_prep_kernel<<<(P + 7) / 8, 256, 0, st>>>(mu, sigma, eps, eps_log, bh, bl, e0, e1, e2, flag, P, D);
         MGP_CHECK_LAUNCH();
-        if (!use_z && !(x_staged & 1)) {
-            tc_x_prep_kernel<<<(unsigned)((N + 7) / 8), 256, 0, st>>>(xhat, ah, al, sn, flag, (int)N, D);
-            MGP_CHECK_LAUNCH();
-        }
+    }
+    if (!use_z && reuse_operands < 2 && !(x_staged & 1)) {
+        tc_x_prep_kernel<<<(unsigned)((N + 7) / 8), 256, 0, st>>>(xhat, ah, al, sn, flag, (int)N, D);
+        MGP_CHECK_LAUNCH();
     }
     if (use_z) return mgp_logprob_tcz_launch(xhat, bh, bl, e0, e1, e2, flag, out, N, P, D, st);
 
@@ -670,7 +647,6 @@ int mgp_logprob_tc_launch(const float* xhat, const float* mu, const float* sigma
     // [B,P,HW] through the 3-D map uses image-aligned x tiles (a chunk may not cross an image end)
     const bool tma_bphw = (layout != MGP_OUT_LOGP_NP) && (HW % 4 == 0) && HW >= 32 && HW <= 256 && tma_ok && D <= 128;
     const bool top1 = (layout == MGP_OUT_TOP1_BP);
-    const bool tma_store = (tma_np || tma_bphw) && !top1;
     // image-aligned x tiles (box of 32 rows) for the [B,P,HW] TMA stores and for the top-1 epilogue
     const bool img_tiles = (tma_bphw && !top1) || (top1 && HW >= 32 && HW <= 256 && D <= 128);
     const uint32_t xbox = img_tiles ? 32u : 128u;
@@ -697,7 +673,7 @@ int mgp_logprob_tc_launch(const float* xhat, const float* mu, const float* sigma
     prm.B = B;
     prm.xbox = (int)xbox;
     prm.nti = ((HW + 31) / 32) * 32;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 0;
     MGP_CUDA(cudaGetDevice(&dev));
     MGP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     // teams of 4 CTAs (fewer when there are fewer prototype tiles) share an x tile and write adjacent tiles
@@ -715,9 +691,9 @@ int mgp_logprob_tc_launch(const float* xhat, const float* mu, const float* sigma
     }
     prm.team = team;
     const int grid = n_teams * team;
-    // shared memory: 1 KiB alignment slack + x tile(s) + prototype stages [+ 32 KiB TMA-store staging] + 2 KiB misc
+    // shared memory: 1 KiB alignment slack + x tile(s) + prototype stages + 32 KiB staging + 2 KiB misc
     const size_t x_max = (size_t)(assume_iso && D > 128 ? 512 : 1024) * D;   // general: 128 x 2D x 4 B (isotropic: half)
-    if (1024 + x_max + (size_t)2 * 2 * SUB_BYTES + (tma_store ? STAGING_BYTES : 0) + 2048 > (size_t)227 * 1024)
+    if (1024 + x_max + (size_t)2 * 2 * SUB_BYTES + STAGING_BYTES + 2048 > (size_t)227 * 1024)
         return MGP_ERR_UNSUPPORTED;
     const size_t smem = (size_t)227 * 1024;
     prm.smem_bytes = (uint32_t)smem;

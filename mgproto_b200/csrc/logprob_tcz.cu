@@ -1,31 +1,24 @@
-// a2 (compute_log_prob, [N,P] output) on the tensor cores with the PATCH tile resident in tensor memory.
+// a2 (compute_log_prob, [N,P] output) on the tensor cores with the PATCH operands resident in registers.
 //
-// logprob_tc.cu feeds both operands of every tcgen05.mma from shared memory and stages the output through shared memory
-// as well; operand fetch + ring writes + the output stage oversubscribe the SM's shared-memory bandwidth (profiles/:
-// 0.65 of the HBM roof for the kernel, 0.52 for the op), and it needs a separate pass that splits x into fp16 hi/lo
-// operands in HBM.  Here:
-//   * the fp32 patch tile [128 x D] is TMA-loaded as it is (no operand pre-pass over x: the split is fused), the eight
-//     epilogue warps convert it in registers to fp16 hi / lo of 256 x and write it with tcgen05.st into TENSOR MEMORY,
-//     where it stays as the A operand (lane = patch) of the 3 * D/16 MMAs of every prototype tile the CTA visits;
-//     |x|^2 of the rank-1 epilogue term is summed in the same pass;
+// logprob_tc.cu feeds both operands of every MMA from shared memory and needs a separate pass that splits x into fp16
+// hi/lo operands in HBM (25.7 MB read, 2 x 25.7 MB written and read back at cfg2).  Here:
+//   * the fp32 patch tile [128 x D] is TMA-loaded as it is (no operand pre-pass over x: the split is fused); each of the
+//     two consumer warpgroups converts its 64-patch slice in registers to fp16 hi / lo of 256 x, laid out as the A
+//     fragments of wgmma.mma_async (RS form), where they stay for the 3 * D/16 MMAs of every prototype tile the CTA
+//     visits with this x tile; |x|^2 of the rank-1 epilogue term is summed in the same pass;
 //   * only the prototype tiles (B operand, the small side: 2 * P * D * 2 bytes in total, L2-resident) stream through a
-//     TMA / mbarrier ring in shared memory: 4 KB of operand reads per MMA instead of 8;
-//   * TMEM lane = patch, column = prototype, so an epilogue thread holds 32 consecutive floats of ONE output row and
-//     hands them, via a 4 KB per-warp block written with eight conflict-free STS.128, to an asynchronous TMA store
-//     (plain LSU stores from only 8 warps per SM back-pressure at ~3.5 TB/s: measured, profiles/);
+//     TMA / mbarrier ring in shared memory; the next fp32 patch tile lands under the current one's MMAs;
+//   * accumulator rows are patches and columns prototypes, so the fragments of a warp are 16 consecutive output rows:
+//     they go, with the affine fix-up, into 128B-swizzled [16 rows x 32 floats] blocks (conflict-free float2 stores)
+//     and out through asynchronous TMA bulk tensor stores (plain stores from the row owners if P % 4 != 0);
 //   * balanced schedule: CTA i owns the pairs [i U / G, (i+1) U / G) of the x-major list of (x tile, prototype tile)
 //     pairs, so every CTA gets U / G pairs +- 1 however the x tiles divide by the grid.
-// The kernel is bound by the HBM write stream of log p (profiles/r2_ka_ablation.txt; DESIGN.md 5.1).
 //
 // Shapes: sigma constant over d inside every prototype (inner dimension K = D; the caller asserts it, the kernel traps
-// if the prototype pre-pass says otherwise) and D in {64, 128, 256}: 2 * 128 accumulator columns + the operand buffers
-// must fit the 512 TMEM columns -- two buffers of D columns for D <= 128 (the next tile is converted under the MMAs of
-// the current one), ONE buffer of 256 columns for D = 256 (the fp32 tile then lands and is converted in two halves,
-// after the current tile's MMAs have retired).  Everything else takes logprob_tc.cu.
+// if the prototype pre-pass says otherwise) and D in {64, 128}: the hi / lo fragments of a 64 x D slice take D / 2
+// registers per thread next to the 64 of the accumulator.  Everything else takes logprob_tc.cu.
 //
-// Warps: 0 prototype TMA producer | 1 MMA issuer (one thread, TS form: A from TMEM) | 2 TMEM allocator + x TMA producer
-//        | 3 idle | 4..11 converter + epilogue: warp = TMEM lane quarter (w & 3); group (w >> 2) converts one column half
-//        of the patch tile and drains one of the two accumulators (alternate prototype tiles).
+// Warps: 0-7 two consumer warpgroups (convert, MMA, epilogue) | 8 prototype TMA producer | 9 patch-tile TMA producer.
 #include <cuda.h>
 #include <cuda_fp16.h>
 
@@ -35,13 +28,13 @@
 namespace {
 using namespace mgp_tc;
 
-constexpr int ZT = 384;            // threads
-constexpr int PT = 128;            // prototypes per tile (UMMA N)
-constexpr int XT = 128;            // patches per tile (UMMA M, TMEM lanes)
+constexpr int ZT = 320;            // threads
+constexpr int PT = 128;            // prototypes per tile (wgmma N)
+constexpr int XT = 128;            // patches per tile (two warpgroups x m64)
 constexpr int KB = 64;             // K elements per prototype smem block (128 B rows)
 constexpr int PSUB = PT * KB * 2;  // one [128 x 64] fp16 block = 16 KiB
+constexpr int STG = 2048;          // one [16 rows x 32 floats] output block; two per consumer warp
 constexpr float X_SCALE = 256.0f;
-constexpr int MAXT = 16;           // prototype tiles per CTA whose epilogue constants are cached in shared memory
 
 struct ZParams {
     const float* e0;
@@ -49,26 +42,20 @@ struct ZParams {
     const float* e2;
     const int* noniso;
     float* out;
-    int N, P, D;
+    int N, P;
     int n_xtiles, n_ptiles;
-    int team;                      // CTAs per team: they share an x tile and take prototype tiles k, k + team, ...
-    int balanced;                  // 1: team = 1 and CTA i owns the pairs [i U / G, (i+1) U / G) of the x-major list of the
-                                   //    U = x tiles * prototype tiles (x tile, prototype tile) pairs -- every CTA gets U / G
-                                   //    pairs +- 1 however the x tiles divide by the grid (a CTA may start / end mid-row)
     int stages;                    // prototype ring depth
-    int debug;                     // ablation (MGP_TC_DEBUG): 1 no global stores, 4 no MMAs, 8 no operand conversion, 16 no prototype loads
 };
 
-__device__ __forceinline__ void tc_mma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                              uint32_t accumulate) {
+// D[64 x 128] (+)= A[64 x 16] (registers: the m64k16 fp16 fragment, 4 x 2 halves) . B[16 x 128] (shared memory)
+__device__ __forceinline__ void wg_mma_rs_n128(float (&d)[64], const uint32_t (&a)[4], uint64_t b_desc) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, 1, 1, 1, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc));
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+
 __device__ __forceinline__ uint32_t pack_h2(__half a, __half b) {
     return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
 }
@@ -79,13 +66,10 @@ logprob_z_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
                  const __grid_constant__ CUtensorMap map_pl, const __grid_constant__ CUtensorMap map_out,
                  const ZParams prm) {
     constexpr int NKB = D / KB;                    // prototype K blocks per tile
+    constexpr int NKS = D / 16;                    // k16 steps
     constexpr int NXB = D / 32;                    // fp32 landing blocks of [128 rows x 32 floats] (128 B rows, swizzled)
-    constexpr int XLB = NXB < 4 ? NXB : 4;         // ... of which the landing buffer holds at most 4 (64 KiB):
-    constexpr int NPH = NXB / XLB;                 //     a D = 256 patch tile lands and is converted in two phases
     constexpr uint32_t XB_BYTES = XT * 128;        // 16 KiB
-    constexpr uint32_t X_BYTES = XLB * XB_BYTES;   // fp32 landing buffer
-    constexpr int ACOLS = D;                       // TMEM columns of one A buffer: D/2 (hi) + D/2 (lo)
-    constexpr int NAB = (D <= 128) ? 2 : 1;        // A buffers in tensor memory: 2 x 128 accumulator columns + NAB x ACOLS <= 512
+    constexpr uint32_t X_BYTES = NXB * XB_BYTES;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
@@ -93,301 +77,168 @@ logprob_z_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
     const int S = prm.stages;
     const uint32_t o_x = 0;                                    // fp32 landing tile
     const uint32_t o_ring = X_BYTES;                           // S x (proto hi, proto lo)
-    const uint32_t o_stg = o_ring + (uint32_t)S * 2 * PSUB;    // 8 warps x [32 rows x 128 B] transposition blocks
-    const uint32_t o_cst = o_stg + 8 * 4096;                   // [MAXT][3][128] e0 / e1 / e2 of this CTA's prototype tiles
-    const uint32_t o_misc = o_cst + MAXT * 1536;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(bp + o_misc); // full[8] empty[8] xfull xempty afull[2] aempty[2] tfull[2] tempty[2]
-    const uint32_t bar0 = base + o_misc;
+    const uint32_t o_stg = o_ring + (uint32_t)S * 2 * PSUB;    // 8 warps x 2 output blocks
+    const uint32_t o_misc = o_stg + 8 * 2 * STG;
+    const uint32_t bar0 = base + o_misc;                       // full[8] empty[8] xfull xempty
     auto FULL = [&](int i) { return bar0 + 8u * i; };
     auto EMPTY = [&](int i) { return bar0 + 8u * (8 + i); };
     const uint32_t XFULL = bar0 + 8u * 16, XEMPTY = bar0 + 8u * 17;
-    auto AFULL = [&](int i) { return bar0 + 8u * (18 + i); };
-    auto AEMPTY = [&](int i) { return bar0 + 8u * (20 + i); };
-    auto TFULL = [&](int i) { return bar0 + 8u * (22 + i); };
-    auto TEMPTY = [&](int i) { return bar0 + 8u * (24 + i); };
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 26);
-    float* s_snp = reinterpret_cast<float*>(bars + 28);        // [2 A buffers][2 column halves][128] partial |x|^2
-    float* s_e = reinterpret_cast<float*>(bp + o_cst);         // loaded once: a CTA revisits the same <= MAXT tiles for every x tile
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
     if (threadIdx.x == 0) {
-        for (int i = 0; i < 8; ++i) { mbar_init(FULL(i), 1); mbar_init(EMPTY(i), 1); }
+        for (int i = 0; i < 8; ++i) { mbar_init(FULL(i), 1); mbar_init(EMPTY(i), 8); }   // empty: one arrive per consumer warp
         mbar_init(XFULL, 1);
         mbar_init(XEMPTY, 8);
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(AFULL(i), 8);
-            mbar_init(AEMPTY(i), 1);
-            mbar_init(TFULL(i), 1);
-            mbar_init(TEMPTY(i), 4);
-        }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t t_acc = tmem_base;                          // 2 x 128 accumulator columns
-    const uint32_t t_a = tmem_base + 256;                      // 2 x ACOLS columns: [hi D/2 | lo D/2]
 
-    const int TS = prm.team;
-    const int n_teams = gridDim.x / TS, team = blockIdx.x / TS, k0 = blockIdx.x % TS;
-    const int n_ptiles = prm.n_ptiles, n_xtiles = prm.n_xtiles;
-    // schedule: this CTA visits n_my_x x tiles xt_of(c), c = 0.., and for each the prototype tiles
-    // p_begin(c), p_begin(c) + p_step, ... < p_end(c)
-    const bool bal = prm.balanced != 0;
-    const long long n_pairs = (long long)n_xtiles * n_ptiles;
+    const int n_ptiles = prm.n_ptiles;
+    const long long n_pairs = (long long)prm.n_xtiles * n_ptiles;
     const long long u0 = n_pairs * blockIdx.x / gridDim.x, u1 = n_pairs * (blockIdx.x + 1) / gridDim.x;
     const int xt_first = (int)(u0 / n_ptiles), xt_last = (int)((u1 - 1) / n_ptiles);
-    const int n_my_x = bal ? (u1 > u0 ? xt_last - xt_first + 1 : 0)
-                           : ((team < n_teams && k0 < n_ptiles && team < n_xtiles) ? (n_xtiles - team + n_teams - 1) / n_teams : 0);
-    const int p_step = bal ? 1 : TS;
-    auto xt_of = [&](int c) { return bal ? xt_first + c : team + c * n_teams; };
-    auto p_begin = [&](int c) { return bal ? (c == 0 ? (int)(u0 - (long long)xt_first * n_ptiles) : 0) : k0; };
-    auto p_end = [&](int c) { return (bal && xt_first + c == xt_last) ? (int)(u1 - (long long)xt_last * n_ptiles) : n_ptiles; };
-    const bool has_work = n_my_x > 0;
-    const uint32_t idesc = umma_idesc_f16(XT, PT);
-    // The kernel is launched with programmatic stream serialisation behind the prototype pre-pass: everything up to
-    // here, the first patch tile's TMA load and its conversion overlap that pre-pass; whoever READS its outputs
-    // (prototype operand tiles, epilogue constants, the anisotropy flag) first executes griddepcontrol.wait.
+    const int n_my_x = u1 > u0 ? xt_last - xt_first + 1 : 0;
+    auto p_begin = [&](int c) { return c == 0 ? (int)(u0 - (long long)xt_first * n_ptiles) : 0; };
+    auto p_end = [&](int c) { return (xt_first + c == xt_last) ? (int)(u1 - (long long)xt_last * n_ptiles) : n_ptiles; };
 
-    if (!has_work) {
-        // nothing to do (tiny problems)
-    } else if (warp == 2 && lane == 0) {
-        // =========================== x-tile TMA producer (fp32 rows, 128B-swizzled 32-float blocks) ===============
-        int l = 0;                                                           // landing-buffer fills so far
+    if (n_my_x == 0) {
+        // nothing to do for this CTA (tiny problems)
+    } else if (warp == 9 && lane == 0) {
+        // =========================== fp32 patch-tile producer (the next tile lands under the current one's MMAs) =====
         for (int c = 0; c < n_my_x; ++c) {
-            const int xt = xt_of(c);
-            for (int ph = 0; ph < NPH; ++ph, ++l) {
-                if (l > 0) mbar_wait(XEMPTY, (uint32_t)((l - 1) & 1));       // the converters have read the previous fill
-                mbar_expect_tx(XFULL, X_BYTES);
+            if (c > 0) mbar_wait(XEMPTY, (uint32_t)((c - 1) & 1));   // the consumers converted the previous tile
+            mbar_expect_tx(XFULL, X_BYTES);
 #pragma unroll
-                for (int b = 0; b < XLB; ++b)
-                    tma_load_2d(base + o_x + b * XB_BYTES, &map_x, (ph * XLB + b) * 32, xt * XT, XFULL);
-            }
+            for (int b = 0; b < NXB; ++b) tma_load_2d(base + o_x + b * XB_BYTES, &map_x, b * 32, (xt_first + c) * XT, XFULL);
         }
-    } else if (warp == 0 && lane == 0) {
+    } else if (warp == 8 && lane == 0) {
         // =========================== prototype TMA producer ===========================
-        asm volatile("griddepcontrol.wait;" ::: "memory");
         int stage = 0;
         uint32_t phase = 0;
         for (int c = 0; c < n_my_x; ++c)
-            for (int pt = p_begin(c); pt < p_end(c); pt += p_step)
+            for (int pt = p_begin(c); pt < p_end(c); ++pt)
                 for (int kb = 0; kb < NKB; ++kb) {
                     mbar_wait(EMPTY(stage), phase ^ 1u);
-                    if (prm.debug & 16) {
-                        mbar_arrive(FULL(stage));
-                    } else {
-                        mbar_expect_tx(FULL(stage), 2 * PSUB);
-                        const uint32_t dst = base + o_ring + (uint32_t)stage * 2 * PSUB;
-                        tma_load_2d(dst, &map_ph, D + kb * KB, pt * PT, FULL(stage));    // the [-2 w mu] half of [P, 2D]
-                        tma_load_2d(dst + PSUB, &map_pl, D + kb * KB, pt * PT, FULL(stage));
-                    }
+                    mbar_expect_tx(FULL(stage), 2 * PSUB);
+                    const uint32_t dst = base + o_ring + (uint32_t)stage * 2 * PSUB;
+                    tma_load_2d(dst, &map_ph, D + kb * KB, pt * PT, FULL(stage));    // the [-2 w mu] half of [P, 2D]
+                    tma_load_2d(dst + PSUB, &map_pl, D + kb * KB, pt * PT, FULL(stage));
                     if (++stage == S) { stage = 0; phase ^= 1u; }
                 }
-    } else if (warp == 1 && lane == 0) {
-        // =========================== MMA issuer (A = patch tile in TMEM, B = prototype block in smem) ===============
-        int stage = 0, acc = 0;
-        uint32_t phase = 0, acc_par = 0;
+    } else if (warp < 8) {
+        // =========================== consumers ===========================
+        if (*reinterpret_cast<const volatile int*>(prm.noniso) != 0) __trap();   // the caller asserted isotropic sigma
+        const int wg = warp >> 2, wq = warp & 3, g = lane >> 2, t = lane & 3;
+        const int rA = wg * 64 + wq * 16 + g;                    // this thread's patch rows of the tile: rA, rA + 8
+        const bool tma_out = (prm.P & 3) == 0;                   // row pitch must be a multiple of 16 B
+        int stage = 0, sbuf = 0;
+        uint32_t phase = 0;
         for (int c = 0; c < n_my_x; ++c) {
-            const int ab = c % NAB;
-            mbar_wait(AFULL(ab), (uint32_t)((c / NAB) & 1));
-            tc_fence_after();
-            const uint32_t a_hi = t_a + (uint32_t)ab * ACOLS, a_lo = a_hi + D / 2;
-            for (int pt = p_begin(c); pt < p_end(c); pt += p_step) {
-                mbar_wait(TEMPTY(acc), acc_par ^ 1u);
-                tc_fence_after();
-                const uint32_t d_tmem = t_acc + (uint32_t)(acc * 128);
+            const int row0 = (xt_first + c) * XT;
+            // ---- fused operand split: fp32 landing tile -> A fragments (hi, lo of 256 x) + |x|^2 of rows rA, rA + 8
+            uint32_t ah[NKS][4], al[NKS][4];
+            float ssA = 0.f, ssB = 0.f;
+            mbar_wait(XFULL, (uint32_t)(c & 1));
+#pragma unroll
+            for (int ks = 0; ks < NKS; ++ks) {
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {                    // fragment register q: row rA + 8 (q & 1), k 16 ks + 2 t + 8 (q >> 1)
+                    const int r = rA + 8 * (q & 1), col = 16 * ks + 2 * t + 8 * (q >> 1), w = col & 31;
+                    const float2 v = *reinterpret_cast<const float2*>(
+                        bp + o_x + (uint32_t)(col >> 5) * XB_BYTES + (uint32_t)r * 128u + ((((w >> 2) ^ (r & 7)) & 7) << 4) + (w & 3) * 4);
+                    if (q & 1) ssB = fmaf(v.x, v.x, fmaf(v.y, v.y, ssB)); else ssA = fmaf(v.x, v.x, fmaf(v.y, v.y, ssA));
+                    const float s0 = v.x * X_SCALE, s1 = v.y * X_SCALE;
+                    const __half h0 = __float2half_rn(s0), h1 = __float2half_rn(s1);
+                    ah[ks][q] = pack_h2(h0, h1);
+                    al[ks][q] = pack_h2(__float2half_rn(s0 - __half2float(h0)), __float2half_rn(s1 - __half2float(h1)));
+                }
+            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(XEMPTY);                  // landing tile consumed: the next one may land
+            ssA += __shfl_xor_sync(0xffffffffu, ssA, 1); ssA += __shfl_xor_sync(0xffffffffu, ssA, 2);
+            ssB += __shfl_xor_sync(0xffffffffu, ssB, 1); ssB += __shfl_xor_sync(0xffffffffu, ssB, 2);
+            for (int pt = p_begin(c); pt < p_end(c); ++pt) {
+                float acc[64];
+#pragma unroll
+                for (int j = 0; j < 64; ++j) acc[j] = 0.f;
                 for (int kb = 0; kb < NKB; ++kb) {
                     mbar_wait(FULL(stage), phase);
-                    tc_fence_after();
                     const uint32_t ph = base + o_ring + (uint32_t)stage * 2 * PSUB, pl = ph + PSUB;
+                    wg_fence();
 #pragma unroll
                     for (int k = 0; k < KB / 16; ++k) {
-                        if (prm.debug & 4) continue;
-                        const uint32_t ac = (uint32_t)(kb * (KB / 2) + k * 8);           // 16 fp16 = 8 TMEM columns
-                        const uint64_t b_h = umma_desc(ph + (uint32_t)k * 32u), b_l = umma_desc(pl + (uint32_t)k * 32u);
-                        tc_mma_f16_ts(d_tmem, a_hi + ac, b_h, idesc, (kb | k) != 0);
-                        tc_mma_f16_ts(d_tmem, a_lo + ac, b_h, idesc, 1u);
-                        tc_mma_f16_ts(d_tmem, a_hi + ac, b_l, idesc, 1u);
+                        const int ks = (kb * KB) / 16 + k;
+                        const uint64_t b_h = gmma_desc(ph + (uint32_t)k * 32u), b_l = gmma_desc(pl + (uint32_t)k * 32u);
+                        wg_mma_rs_n128(acc, ah[ks], b_h);
+                        wg_mma_rs_n128(acc, al[ks], b_h);
+                        wg_mma_rs_n128(acc, ah[ks], b_l);
                     }
-                    tc_commit(EMPTY(stage));
+                    wg_commit();
+                    wg_wait0();
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(EMPTY(stage));    // this warp no longer reads the stage
                     if (++stage == S) { stage = 0; phase ^= 1u; }
                 }
-                tc_commit(TFULL(acc));
-                acc ^= 1;
-                if (acc == 0) acc_par ^= 1u;
-            }
-            tc_commit(AEMPTY(ab));                                                       // this A buffer may be overwritten
-        }
-    } else if (warp >= 4) {
-        // =========================== converter + epilogue ===========================
-        const int e = warp - 4, q = e & 3, h = e >> 2;
-        const int row = q * 32 + lane;                                                    // TMEM lane = patch row of the tile
-        const uint32_t lane_off = (uint32_t)(q * 32) << 16;
-        // fp32 landing tile -> fp16 hi / lo of 256 x in TMEM (A buffer `ab`), |x|^2 -> s_sn[ab]
-        auto convert = [&](int cc) {
-            const int ab = cc % NAB;
-            float ss = 0.f;
-            constexpr int HB = XLB / 2;                                                   // landing blocks of this group per fill
-#pragma unroll 1
-            for (int ph = 0; ph < NPH; ++ph) {
-            mbar_wait(XFULL, (uint32_t)((cc * NPH + ph) & 1));
-            if (ph == 0 && cc >= NAB) {
-                mbar_wait(AEMPTY(ab), (uint32_t)(((cc / NAB) - 1) & 1));                  // the MMAs that read this buffer are done
-                tc_fence_after();
-            }
+                // ---- epilogue: log p = e0 + e1 acc + e2 |x|^2, 4 blocks of [16 patches x 32 prototypes] per warp
 #pragma unroll
-            for (int bb = 0; bb < ((prm.debug & 8) ? 0 : HB); ++bb) {
-                const uint8_t* blk = bp + o_x + (uint32_t)(h * HB + bb) * XB_BYTES + (uint32_t)row * 128u;
-                uint32_t hi[16], lo[16];
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const float4 v = *reinterpret_cast<const float4*>(blk + (((j ^ (row & 7)) & 7) << 4));
-                    const float a[4] = {v.x, v.y, v.z, v.w};
-                    __half hh[4], ll[4];
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        ss = fmaf(a[i], a[i], ss);
-                        const float s1 = a[i] * X_SCALE;
-                        hh[i] = __float2half_rn(s1);
-                        ll[i] = __float2half_rn(s1 - __half2float(hh[i]));
-                    }
-                    hi[2 * j] = pack_h2(hh[0], hh[1]); hi[2 * j + 1] = pack_h2(hh[2], hh[3]);
-                    lo[2 * j] = pack_h2(ll[0], ll[1]); lo[2 * j + 1] = pack_h2(ll[2], ll[3]);
-                }
-                // 32 elements = 16 TMEM columns per landing block; element k of the row -> column k / 2
-                const uint32_t col = (uint32_t)((ph * XLB + h * HB + bb) * 16);
-                asm volatile(
-                    "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-                    ::"r"(t_a + (uint32_t)ab * ACOLS + col + lane_off), "r"(hi[0]), "r"(hi[1]), "r"(hi[2]), "r"(hi[3]), "r"(hi[4]),
-                      "r"(hi[5]), "r"(hi[6]), "r"(hi[7]), "r"(hi[8]), "r"(hi[9]), "r"(hi[10]), "r"(hi[11]), "r"(hi[12]), "r"(hi[13]),
-                      "r"(hi[14]), "r"(hi[15])
-                    : "memory");
-                asm volatile(
-                    "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-                    ::"r"(t_a + (uint32_t)ab * ACOLS + D / 2 + col + lane_off), "r"(lo[0]), "r"(lo[1]), "r"(lo[2]), "r"(lo[3]),
-                      "r"(lo[4]), "r"(lo[5]), "r"(lo[6]), "r"(lo[7]), "r"(lo[8]), "r"(lo[9]), "r"(lo[10]), "r"(lo[11]), "r"(lo[12]),
-                      "r"(lo[13]), "r"(lo[14]), "r"(lo[15])
-                    : "memory");
-            }
-            if (ph + 1 < NPH) {                                                          // landing buffer consumed: next fill may start
-                __syncwarp();
-                if (lane == 0) mbar_arrive(XEMPTY);
-            }
-            }
-            s_snp[(ab * 2 + h) * 128 + row] = ss;                                        // (summed by the reader after the tile's barrier)
-            tmem_st_wait();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                mbar_arrive(XEMPTY);                                                      // landing tile consumed
-                mbar_arrive(AFULL(ab));                                                   // operand (this warp's share) in TMEM
-            }
-        };
-        int acc = 0;
-        uint32_t acc_par = 0;
-        convert(0);
-        asm volatile("griddepcontrol.wait;" ::: "memory");
-        if (*reinterpret_cast<const volatile int*>(prm.noniso) != 0) __trap();            // the caller asserted isotropic sigma
-        for (int i = threadIdx.x - 128; i < MAXT * 128; i += 256) {                       // epilogue constants of my tiles k0, k0+TS, ...
-            const int ti = i >> 7, pt = k0 + ti * TS;
-            const int p = pt * PT + (i & 127);
-            const bool ok = pt < n_ptiles && p < prm.P;
-            s_e[ti * 384 + (i & 127)] = ok ? prm.e0[p] : 0.f;
-            s_e[ti * 384 + 128 + (i & 127)] = ok ? prm.e1[p] : 0.f;
-            s_e[ti * 384 + 256 + (i & 127)] = ok ? prm.e2[p] : 0.f;
-        }
-        for (int c = 0; c < n_my_x; ++c) {
-            const int ab = c % NAB;
-            const int row0 = xt_of(c) * XT;
-            asm volatile("bar.sync 1, 256;" ::: "memory");                                // both halves' |x|^2 of this tile are in
-            const float sn = s_snp[(ab * 2) * 128 + row] + s_snp[(ab * 2 + 1) * 128 + row];
-            const int n = row0 + row;
-            const int n_my = (p_end(c) - p_begin(c) + p_step - 1) / p_step;
-            int ti = 0;
-            for (int pt = p_begin(c); pt < p_end(c); pt += p_step, ++ti) {
-                // the next x tile's operand is converted half-way through this tile's prototype tiles: the first
-                // accumulators are drained first (the MMA warp is never held up), and the operand is ready well before
-                // the last prototype tile of this x tile has been issued
-                // (the two warp groups convert one tile apart, so that one of them keeps draining / storing)
-                if (NAB == 2 && ti == min(n_my / 2 + h, n_my - 1) && c + 1 < n_my_x) convert(c + 1);
-                // the two warp groups drain alternate accumulators (tiles): each has two MMA tile times per tile
-                if (acc != h) { acc ^= 1; continue; }
-                mbar_wait(TFULL(acc), acc_par);
-                tc_fence_after();
-                const float* se = s_e + ((pt - k0) / TS) * 384;
-#pragma unroll 1
                 for (int ch = 0; ch < 4; ++ch) {
-                    const int c0 = ch * 32;                                               // prototype columns [c0, c0+32) of the tile
-                    uint32_t r[32];
-                    tmem_ld32(t_acc + (uint32_t)(acc * 128 + c0) + lane_off, r);
-                    tmem_ld_wait();
-                    if (ch == 3) {                                                        // accumulator slice in registers: release it
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(TEMPTY(acc));
-                    }
-                    const int p0 = pt * PT + c0;
-                    const bool tma_out = (prm.P & 3) == 0;                            // row pitch must be a multiple of 16 B
-                    if (p0 >= prm.P || (prm.debug & 1)) continue;
-                    if (!tma_out && n >= prm.N) continue;
-                    float* dst = prm.out + (size_t)n * prm.P + p0;
-                    float v[32];
-#pragma unroll
-                    for (int j4 = 0; j4 < 8; ++j4) {
-                        const float4 c0v = *reinterpret_cast<const float4*>(se + c0 + 4 * j4);
-                        const float4 c1v = *reinterpret_cast<const float4*>(se + 128 + c0 + 4 * j4);
-                        const float4 c2v = *reinterpret_cast<const float4*>(se + 256 + c0 + 4 * j4);
-                        v[4 * j4 + 0] = fmaf(c1v.x, __uint_as_float(r[4 * j4 + 0]), fmaf(c2v.x, sn, c0v.x));
-                        v[4 * j4 + 1] = fmaf(c1v.y, __uint_as_float(r[4 * j4 + 1]), fmaf(c2v.y, sn, c0v.y));
-                        v[4 * j4 + 2] = fmaf(c1v.z, __uint_as_float(r[4 * j4 + 2]), fmaf(c2v.z, sn, c0v.z));
-                        v[4 * j4 + 3] = fmaf(c1v.w, __uint_as_float(r[4 * j4 + 3]), fmaf(c2v.w, sn, c0v.w));
-                    }
+                    const int p0 = pt * PT + ch * 32;
+                    // epilogue constants of prototype column p (read per n8 block: keeps them out of the live set)
+                    auto ev = [&](int p, float& c0, float& c1, float& c2) {
+                        const bool ok = p < prm.P;
+                        c0 = ok ? __ldg(prm.e0 + p) : 0.f;
+                        c1 = ok ? __ldg(prm.e1 + p) : 0.f;
+                        c2 = ok ? __ldg(prm.e2 + p) : 0.f;
+                    };
                     if (tma_out) {
-                        // [32 rows x 128 B] block in the tensor map's 128B-swizzle layout (lane = row writes its 128 B,
-                        // 16-byte chunks XOR-ed with the row: conflict-free) -> one asynchronous TMA store; rows / columns
-                        // outside [N, P] are clipped by the map.  The block is reused once the previous store has READ it.
-                        uint8_t* stg = bp + o_stg + e * 4096;
-                        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+                        uint8_t* stg = bp + o_stg + (uint32_t)(warp * 2 + sbuf) * STG;
+                        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");   // this block's previous store has read it
                         __syncwarp();
 #pragma unroll
-                        for (int j = 0; j < 8; ++j)
-                            *reinterpret_cast<float4*>(stg + lane * 128 + (((j ^ (lane & 7)) & 7) << 4)) =
-                                make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+                        for (int i = 0; i < 4; ++i) {
+                            const int cc = 8 * i + 2 * t;
+                            float a0, a1, a2, b0, b1, b2;
+                            ev(p0 + cc, a0, a1, a2);
+                            ev(p0 + cc + 1, b0, b1, b2);
+#pragma unroll
+                            for (int rr = 0; rr < 2; ++rr) {
+                                const int idx = 4 * (4 * ch + i) + 2 * rr, r16 = g + 8 * rr;
+                                const float sn = rr ? ssB : ssA;
+                                const float v0 = fmaf(a1, acc[idx], fmaf(a2, sn, a0));
+                                const float v1 = fmaf(b1, acc[idx + 1], fmaf(b2, sn, b0));
+                                *reinterpret_cast<float2*>(stg + r16 * 128 + ((((cc >> 2) ^ (r16 & 7)) & 7) << 4) + (cc & 3) * 4) =
+                                    make_float2(v0, v1);
+                            }
+                        }
                         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
                         __syncwarp();
                         if (lane == 0) {
-                            tma_store_2d(&map_out, smem_u32(stg), p0, row0 + q * 32);
+                            tma_store_2d(&map_out, smem_u32(stg), p0, row0 + wg * 64 + wq * 16);
                             asm volatile("cp.async.bulk.commit_group;" ::: "memory");
                         }
+                        sbuf ^= 1;
                     } else {
 #pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (p0 + j < prm.P) dst[j] = v[j];
+                        for (int i = 0; i < 4; ++i)
+#pragma unroll
+                            for (int rr = 0; rr < 2; ++rr)
+#pragma unroll
+                                for (int j = 0; j < 2; ++j) {
+                                    const int n = row0 + rA + 8 * rr, p = p0 + 8 * i + 2 * t + j;
+                                    const float sn = rr ? ssB : ssA;
+                                    float c0, c1, c2;
+                                    ev(p, c0, c1, c2);
+                                    if (n < prm.N && p < prm.P)
+                                        prm.out[(size_t)n * prm.P + p] = fmaf(c1, acc[4 * (4 * ch + i) + 2 * rr + j], fmaf(c2, sn, c0));
+                                }
                     }
                 }
-                acc ^= 1;
-                acc_par ^= 1u;                                                            // my accumulator comes round every other tile
             }
-            // one A buffer (D = 256): the next tile's operand can only be written once this tile's MMAs have retired
-            if (NAB == 1 && c + 1 < n_my_x) convert(c + 1);
         }
-    }
-    if (warp >= 4 && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // my TMA stores have landed
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
+        if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // my TMA stores have landed
     }
 }
 
-// x [N, D] fp32 row-major, box = 32 floats x 128 rows, 128 B swizzle; out-of-bounds rows read as zero
 bool make_map_x(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols) {
     EncodeTiledFn enc = get_encode();
     if (!enc) return false;
@@ -400,13 +251,13 @@ bool make_map_x(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols) {
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// output [N, P] fp32 row-major, box = 32 prototypes x 32 patches, 128 B swizzle (the inner box is exactly one 128 B row)
+// output [N, P] fp32, box = 32 prototypes x 16 patches, 128B swizzle (inner box = 128 B)
 bool make_map_out(CUtensorMap* m, const void* ptr, uint64_t N, uint64_t P) {
     EncodeTiledFn enc = get_encode();
     if (!enc) return false;
     cuuint64_t dims[2] = {P, N};
     cuuint64_t strides[1] = {P * 4};
-    cuuint32_t box[2] = {32, 32};
+    cuuint32_t box[2] = {32, 16};
     cuuint32_t es[2] = {1, 1};
     return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(ptr), dims, strides, box, es,
                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
@@ -415,9 +266,8 @@ bool make_map_out(CUtensorMap* m, const void* ptr, uint64_t N, uint64_t P) {
 
 }  // namespace
 
-bool mgp_logprob_tcz_supported(int P, int D) { return (D == 64 || D == 128 || D == 256) && P >= 1 && get_encode() != nullptr; }
+bool mgp_logprob_tcz_supported(int P, int D) { return (D == 64 || D == 128) && P >= 1 && get_encode() != nullptr; }
 
-// bh / bl [P, 2D] fp16, e0 / e1 / e2 [P], noniso: the prototype-side workspace of logprob_tc.cu (tc_proto_prep_kernel)
 int mgp_logprob_tcz_launch(const float* xhat, const void* bh, const void* bl, const float* e0, const float* e1,
                            const float* e2, const int* noniso, float* out, long long N, int P, int D, cudaStream_t st) {
     CUtensorMap mx, mph, mpl, mout;
@@ -431,69 +281,28 @@ int mgp_logprob_tcz_launch(const float* xhat, const void* bh, const void* bl, co
         return MGP_ERR_UNSUPPORTED;
     ZParams prm;
     prm.e0 = e0; prm.e1 = e1; prm.e2 = e2; prm.noniso = noniso; prm.out = out;
-    prm.N = (int)N; prm.P = P; prm.D = D;
+    prm.N = (int)N; prm.P = P;
     prm.n_xtiles = (int)((N + XT - 1) / XT);
     prm.n_ptiles = (P + PT - 1) / PT;
-    const char* dbg = getenv("MGP_TC_DEBUG");
-    prm.debug = dbg ? atoi(dbg) : 0;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 0;
     MGP_CUDA(cudaGetDevice(&dev));
     MGP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    // CTAs per team (sharing an x tile): rounds = ceil(x tiles / teams) * ceil(prototype tiles / team); the smallest
-    // team within 10 % of the best count wins (measured at cfg2: one CTA per x tile is 4-5 % faster than teams of 4)
-    int team = 1;
-    {
-        long best = -1;
-        for (int t = 1; t <= 8; t *= 2) {
-            if (t > prm.n_ptiles || t > sms) break;
-            int nt = sms / t;
-            if (nt > prm.n_xtiles) nt = prm.n_xtiles;
-            const long cost = (long)((prm.n_xtiles + nt - 1) / nt) * ((prm.n_ptiles + t - 1) / t);
-            if (best < 0 || cost * 10 < best * 9) { best = cost; team = t; }
-        }
-    }
-    const char* ts = getenv("MGP_TC_TEAM");
-    if (ts && atoi(ts) > 0) team = atoi(ts);
-    if (team > prm.n_ptiles) team = prm.n_ptiles;
-    if (team > sms) team = sms;
-    int n_teams = sms / team;
-    if (n_teams > prm.n_xtiles) n_teams = prm.n_xtiles;
-    const size_t x_bytes = (size_t)XT * (D < 128 ? D : 128) * 4;       // landing buffer: at most 4 blocks of 32 floats
-    while ((prm.n_ptiles + team - 1) / team > MAXT) ++team;              // every CTA caches its tiles' epilogue constants
-    n_teams = sms / team;
-    if (n_teams > prm.n_xtiles) n_teams = prm.n_xtiles;
-    if (n_teams < 1) return MGP_ERR_UNSUPPORTED;
-    // balanced pair schedule whenever one CTA can cache every prototype tile's constants (MGP_TC_TEAM forces the team schedule)
-    const bool balanced = !(ts && atoi(ts) > 0) && prm.n_ptiles <= MAXT;
-    if (balanced) team = 1;
-    prm.team = team;
-    prm.balanced = balanced ? 1 : 0;
-    int stages = (int)((227 * 1024 - 1024 - 4096 - MAXT * 1536 - 8 * 4096 - x_bytes) / (2 * PSUB));
+    const size_t x_bytes = (size_t)XT * D * 4;
+    int stages = (int)((227 * 1024 - 1024 - 256 - 8 * 2 * STG - x_bytes) / (2 * PSUB));
     if (stages > 8) stages = 8;
     if (stages < 2) return MGP_ERR_UNSUPPORTED;
     prm.stages = stages;
     const long long n_pairs = (long long)prm.n_xtiles * prm.n_ptiles;
-    const int grid = balanced ? (int)(n_pairs < sms ? n_pairs : sms) : n_teams * team;
-    const size_t smem = 1024 + x_bytes + (size_t)stages * 2 * PSUB + 8 * 4096 + MAXT * 1536 + 4096;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(ZT);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;      // start under the tail of the prototype pre-pass
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    if (D == 256) {
-        MGP_CUDA(cudaFuncSetAttribute(logprob_z_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        MGP_CUDA(cudaLaunchKernelEx(&cfg, logprob_z_kernel<256>, mx, mph, mpl, mout, prm));
-    } else if (D == 128) {
-        MGP_CUDA(cudaFuncSetAttribute(logprob_z_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        MGP_CUDA(cudaLaunchKernelEx(&cfg, logprob_z_kernel<128>, mx, mph, mpl, mout, prm));
-    } else {
-        MGP_CUDA(cudaFuncSetAttribute(logprob_z_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        MGP_CUDA(cudaLaunchKernelEx(&cfg, logprob_z_kernel<64>, mx, mph, mpl, mout, prm));
-    }
+    const int grid = (int)(n_pairs < sms ? n_pairs : sms);
+    const size_t smem = 1024 + x_bytes + (size_t)stages * 2 * PSUB + 8 * 2 * STG + 256;
+#define MGP_Z_LAUNCH(DD)                                                                                           \
+    do {                                                                                                           \
+        MGP_CUDA(cudaFuncSetAttribute(logprob_z_kernel<DD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+        logprob_z_kernel<DD><<<grid, ZT, smem, st>>>(mx, mph, mpl, mout, prm);                                     \
+    } while (0)
+    if (D == 64) MGP_Z_LAUNCH(64);
+    else MGP_Z_LAUNCH(128);
+#undef MGP_Z_LAUNCH
+    MGP_CHECK_LAUNCH();
     return MGP_OK;
 }

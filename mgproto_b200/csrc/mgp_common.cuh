@@ -1,4 +1,4 @@
-// Shared helpers for the mgproto_b200 kernels (sm_100a).
+// Shared helpers for the mgproto_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -47,13 +47,7 @@ __device__ __forceinline__ unsigned long long top1_pack(float v, int hw) {
     return ((unsigned long long)f2key(v) << 32) | (unsigned long long)(0xffffffffu - (unsigned)hw);
 }
 
-// two fp32 FMAs in one issue slot (sm_100a FFMA2): d = a * b + c lane-wise, each lane an IEEE fma
+// d = a * b + c lane-wise, each lane an IEEE fma (two FFMA on sm_90a)
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-    float2 d;
-    asm("{\n\t.reg .b64 ra, rb, rc, rd;\n\t"
-        "mov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tmov.b64 rc, {%6, %7};\n\t"
-        "fma.rn.f32x2 rd, ra, rb, rc;\n\tmov.b64 {%0, %1}, rd;\n\t}"
-        : "=f"(d.x), "=f"(d.y)
-        : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y), "f"(c.x), "f"(c.y));
-    return d;
+    return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }

@@ -1,5 +1,5 @@
-// Inline PTX for the sm_100a tensor-core / TMA / mbarrier path, shared by logprob_tc.cu and em_tc.cu.
-// SASS: tcgen05.mma -> UTCHMMA, tcgen05.ld -> LDTM, cp.async.bulk.tensor -> UTMALDG / UTMASTG, mbarrier -> SYNCS.
+// Inline PTX for the sm_90a tensor-core / TMA / mbarrier path, shared by logprob_tc.cu and em_tc.cu.
+// SASS: wgmma.mma_async -> HGMMA, cp.async.bulk.tensor -> UTMALDG / UTMASTG, mbarrier -> SYNCS.
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
@@ -51,58 +51,49 @@ __device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t sr
                  ::"l"(map), "r"(src), "r"(c0), "r"(c1), "r"(c2)
                  : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                           uint32_t accumulate) {
+// Warpgroup MMA (sm_90a wgmma.mma_async): fp16 x fp16 -> fp32, both operands from shared memory, the accumulator in
+// the registers of the issuing warpgroup.  Fragment of an m64nN accumulator, warp w (of the warpgroup), lane l:
+// d[4 i + 2 h + j] = D[16 w + l / 4 + 8 h][8 i + 2 (l % 4) + j].
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// D[64 x 32] (+)= A[64 x 16] . B[16 x 32]; TA = 1: A is MN-major (transposed) in shared memory
+template <int TA>
+__device__ __forceinline__ void wg_mma_n32(float (&d)[16], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TA));
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
+// D[64 x 16] (+)= A[64 x 16] . B[16 x 16]
+template <int TA>
+__device__ __forceinline__ void wg_mma_n16(float (&d)[8], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TA));
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// Shared-memory matrix descriptors (cute::UMMA::SmemDescriptor, sm_100): start>>4 at [0,14), LBO>>4 at [16,30),
-// SBO>>4 at [32,46), version 1 at [46,48), layout SWIZZLE_128B (2) at [61,64).
-//   K-major, SWIZZLE_128B : 8-row groups of 128 B rows (1024 B) -> SBO = 1024 B; LBO unused (1)
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+// Shared-memory matrix descriptors (sm_90 GMMA): start>>4 at [0,14), LBO>>4 at [16,30), SBO>>4 at [32,46),
+// layout SWIZZLE_128B (1) at [62,64).
+//   K-major, SWIZZLE_128B : 8-row groups of 128 B rows (1024 B) -> SBO = 1024 B; LBO unused (1).  A K step of 16
+//   fp16 inside the 128 B row advances the start address by 32 B.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr) {
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
 //   MN-major, SWIZZLE_128B (canonical ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units): 64 MN-elements (128 B)
 //   contiguous, the next 64 at +LBO; 8 k-rows at 128 B stride, the next 8 at +SBO
-__device__ __forceinline__ uint64_t umma_desc_mn(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+__device__ __forceinline__ uint64_t gmma_desc_mn(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) |
-           ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) | (1ull << 46) | (2ull << 61);
-}
-// kind::f16 instruction descriptor: D = f32 (1 << 4), A = B = f16 (0), a_major at bit 15, b_major at bit 16
-// (0 = K-major, 1 = MN-major), N >> 3 at [17,23), M >> 4 at [24,29)
-__device__ __forceinline__ uint32_t umma_idesc_f16(int m, int n, int a_mn_major = 0, int b_mn_major = 0) {
-    return (1u << 4) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) | ((uint32_t)(n >> 3) << 17) |
-           ((uint32_t)(m >> 4) << 24);
+           ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) | (1ull << 62);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,

@@ -1,4 +1,4 @@
-"""MGProto with a B200-native prototype head -- the drop-in boundary (SURVEY.md section 8b).
+"""MGProto with a CUDA-native (H100) prototype head -- the drop-in boundary (SURVEY.md section 8b).
 
 Same constructor, methods, attributes and state-dict keys as the reference's ``model.MGProto``
 (``/root/reference/model.py:77-482``), so the reference's ``train_and_test.py`` / ``push.py`` /
@@ -9,7 +9,7 @@ custom ``features``; ``construct_MGProto(pretrained=True)`` loads weights from `
 otherwise warns and keeps the random initialisation (no network on the target boxes).  The backbone, add-on convs, embedding and losses are
 ordinary PyTorch; everything between the add-on output ``[B,D,H,W]`` and the log mixture
 evidences ``[B,C,T]`` -- plus the memory bank and its EM update -- runs in the hand-written
-sm_100a kernels of ``libmgproto_b200.so``.  There is no CPU path: tensors must be on a CUDA
+sm_90a kernels of ``libmgproto_b200.so``.  There is no CPU path: tensors must be on a CUDA
 device when the hot methods are called.
 """
 from __future__ import annotations
@@ -111,14 +111,13 @@ class MGProto(nn.Module):
         self.alpha = 0.1
         self.tau = 0.990
 
-        # B200 knobs (not in the reference)
-        self.math_mode = "auto"          # 'fp32' exact SIMT | 'tc' tcgen05 fp16x3 | 'auto'
+        # implementation knobs (not in the reference)
+        self.math_mode = "auto"          # 'fp32' exact SIMT | 'tc' wgmma fp16x3 | 'auto'
         self.em_n_split = 2              # row splits of the EM statistics reduction
         self.em_group = None             # torch.distributed process group of the batch-sharded replicas (parallel.py)
         self.em_shard = False            # True: shard bank rows over the ranks + all-reduce the EM statistics per loop
-        self.overlap_enqueue = False     # multi-GPU: True = all-gather + enqueue on a side stream behind the backward (measured
-                                         # slower on 2 x B200: 707 vs 640 us/step, profiles/r2_mgpu_breakdown.txt: the NCCL kernel
-                                         # and the backward kernels delay each other), False = inline on the main stream
+        self.overlap_enqueue = False     # multi-GPU: True = all-gather + enqueue on a side stream behind the backward (the
+                                         # NCCL kernel and the backward kernels delay each other), False = inline on the main stream
         self._side_stream = None
         self._em_status = None           # int32[1] on the device: set by the tensor-core EM kernel if sigma was not isotropic
         self._adam_step_dev = None       # int32[1] on the device: Adam step count, advanced by update_GMM's planner

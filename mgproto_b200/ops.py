@@ -1,7 +1,7 @@
 """Tensor-level wrappers over the C ABI (include/mgproto_b200.h).
 
 PyTorch is plumbing here: it owns device memory and streams; every function validates its
-tensors (CUDA, fp32, contiguous) and enqueues hand-written sm_100a kernels on the current
+tensors (CUDA, fp32, contiguous) and enqueues hand-written sm_90a kernels on the current
 stream through ctypes.  Nothing falls back to ATen or to the CPU.
 """
 from __future__ import annotations
@@ -203,14 +203,14 @@ def logprob(xhat_nd, mu_pd, sigma_pd, layout=MGP_OUT_LOGP_NP, B=None, HW=None, e
     m = _math(math)
     if m == MGP_MATH_AUTO:
         # one cached host check (sigma never changes in the reference's loop): isotropic sigma lets the [N,P] layout
-        # take the TMEM-resident kernel with the fused operand split (D <= 128) and D = 256 fit the tensor-core tiles
+        # take the register-resident kernel with the fused operand split (D <= 128) and D = 256 fit the tensor-core tiles
         iso = sigma_is_isotropic(sg)
         if D > 128:
             m = MGP_MATH_TC_ISO if (D == 256 and iso) else MGP_MATH_FP32
         elif iso and D in (64, 128):
             m = MGP_MATH_TC_ISO
     nbytes = lib.mgp_logprob_ws_bytes(B_, HW_, P, D, m)
-    # The TMEM-resident kernel reads only prototype-side operands from the workspace (fp16 hi/lo tiles, per-prototype
+    # The register-resident kernel reads only prototype-side operands from the workspace (fp16 hi/lo tiles, per-prototype
     # constants): while mu / sigma are unchanged (eval, push, OoD scoring: every batch) the pre-pass is skipped.
     cache_key = None
     if ws is None and m == MGP_MATH_TC_ISO and lib.mgp_logprob_ws_is_prototype_only(int(layout), P, D, m):

@@ -1,5 +1,5 @@
 """Multi-GPU plumbing for the hot path (SURVEY.md section 8e): one process per GPU,
-``torch.distributed`` (NCCL on the B200 box, gloo in CPU tests).
+``torch.distributed`` (NCCL on GPUs, gloo in CPU tests).
 
 The path shards by image: the head (log-likelihood, top-T, logits, backward) touches one
 image's patches against replicated prototypes -- no communication.  Two exchanges keep every

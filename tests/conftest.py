@@ -12,7 +12,7 @@ GOLDEN_CASES = ["tiny", "small_diag", "k10d128"]
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -311,14 +311,14 @@ def test_state_dict_roundtrip(golden):
 
 
 # ---------------------------------------------------------------------------------------------
-# tensor-core log-likelihood kernel (tcgen05, fp16 hi/lo x3) against the exact fp32 SIMT kernel
+# tensor-core log-likelihood kernel (wgmma, fp16 hi/lo x3) against the exact fp32 SIMT kernel
 # and a float64 restatement, at shapes with ragged tiles and at the BASELINE size
 @pytest.mark.parametrize("sigma_mode", ["iso", "diag"])
 @pytest.mark.parametrize("shape", [(3, 49, 130, 64), (5, 196, 2000, 128), (2, 200, 257, 128)])
 def test_logprob_tc_vs_fp32(shape, sigma_mode):
     from mgproto_b200 import ops, _lib
     if not _lib.load().mgp_has_tensor_core_path():
-        pytest.skip("library built without the tcgen05 path")
+        pytest.skip("library built without the tensor-core path")
     B, HW, P, D = shape
     g = torch.Generator().manual_seed(5)
     x = F.normalize(torch.randn(B * HW, D, generator=g), dim=1).to(_dev())
@@ -341,15 +341,15 @@ def test_logprob_tc_vs_fp32(shape, sigma_mode):
 
 @pytest.mark.parametrize("shape", [(3, 49, 130, 64), (5, 196, 2000, 128), (2, 200, 257, 128), (1, 7, 5, 128), (9, 196, 1000, 64),
                                    (2, 196, 300, 256), (7, 49, 2000, 256), (1, 7, 5, 256)])
-def test_logprob_tmem_resident_kernel_vs_fp64(shape):
-    """compute_log_prob's [N,P] kernel with the patch tile resident in tensor memory and the fp16 hi/lo split fused
-    (csrc/logprob_tcz.cu; taken by math='auto' when sigma is isotropic, D <= 256 -- D = 256 keeps ONE operand buffer in
-    tensor memory and lands / converts the patch tile in two halves): ragged tiles on both sides, against
-    float64 and against the kernel that splits x in a pre-pass (csrc/logprob_tc.cu)."""
+def test_logprob_iso_np_vs_fp64(shape):
+    """compute_log_prob's [N,P] kernel with the patch operands resident in registers and the fp16 hi/lo split fused
+    (csrc/logprob_tcz.cu; taken by math='auto' when sigma is isotropic and D <= 128; D = 256 takes csrc/logprob_tc.cu):
+    ragged tiles on both sides (P % 4 != 0 takes the direct-store epilogue), against float64, against the kernel that
+    splits x in a pre-pass (tc_z off: csrc/logprob_tc.cu) and against the exact fp32 SIMT kernel."""
     from mgproto_b200 import ops, _lib
     lib = _lib.load()
     if not lib.mgp_has_tensor_core_path():
-        pytest.skip("library built without the tcgen05 path")
+        pytest.skip("library built without the tensor-core path")
     B, HW, P, D = shape
     g = torch.Generator().manual_seed(11)
     x = F.normalize(torch.randn(B * HW, D, generator=g), dim=1).to(_dev())
@@ -358,22 +358,26 @@ def test_logprob_tmem_resident_kernel_vs_fp64(shape):
     ref64 = (-0.5 * D * np.log(2 * np.pi) - sg.double().log().sum(1)[None, :]
              - 0.5 * (((x.double()[:, None, :] - mu.double()[None]) / sg.double()[None]) ** 2).sum(-1))
     a = ops.logprob(x, mu, sg, 0, math="auto")
+    a2 = ops.logprob(x, mu, sg, 0, math="auto")                        # prototype operands from the cache
     prev = lib.mgp_set_option(b"tc_z", 0)
     try:
         b = ops.logprob(x, mu, sg, 0, math="auto")
     finally:
         lib.mgp_set_option(b"tc_z", prev)
+    f = ops.logprob(x, mu, sg, 0, math="fp32")
     torch.testing.assert_close(a.double(), ref64, rtol=2e-5, atol=2e-5)
     torch.testing.assert_close(a, b, rtol=2e-5, atol=2e-5)
+    torch.testing.assert_close(a, f, rtol=2e-5, atol=2e-5)
+    assert torch.equal(a, a2)
 
 
 def test_logprob_prototype_operands_are_cached_until_the_prototypes_change():
-    """ops.logprob (auto, isotropic sigma, [N,P]) keeps the prototype-side operands of the TMEM-resident kernel while
+    """ops.logprob (auto, isotropic sigma, [N,P]) keeps the prototype-side operands of the register-resident kernel while
     mu / sigma are unchanged (version counter) and rebuilds them after an in-place change -- including update_GMM's
     raw-pointer writes, which bump the counters explicitly."""
     from mgproto_b200 import ops, _lib
     if not _lib.load().mgp_has_tensor_core_path():
-        pytest.skip("library built without the tcgen05 path")
+        pytest.skip("library built without the tensor-core path")
     B, HW, P, D = 4, 49, 300, 128
     g = torch.Generator().manual_seed(5)
     x = F.normalize(torch.randn(B * HW, D, generator=g), dim=1).to(_dev())
@@ -405,7 +409,7 @@ def test_logprob_tc_baseline_size_properties():
     three output layouts with each other (size-independent properties; no CPU oracle at this size)."""
     from mgproto_b200 import ops, _lib
     if not _lib.load().mgp_has_tensor_core_path():
-        pytest.skip("library built without the tcgen05 path")
+        pytest.skip("library built without the tensor-core path")
     B, HW, P, D = 256, 196, 2000, 128
     g = torch.Generator().manual_seed(1)
     x = F.normalize(torch.randn(B * HW, D, generator=g), dim=1).to(_dev())
@@ -415,7 +419,7 @@ def test_logprob_tc_baseline_size_properties():
     rows = torch.arange(0, B * HW, 97, device=_dev())
     ref = -np.pi * ((x[rows].double()[:, None, :] - mu.double()[None]) ** 2).sum(-1)       # KA1
     torch.testing.assert_close(lp[rows].double(), ref, rtol=1e-5, atol=2e-5)
-    lpz = ops.logprob(x, mu, sg, 0, math="auto")                                           # TMEM-resident kernel
+    lpz = ops.logprob(x, mu, sg, 0, math="auto")                                           # register-resident kernel
     torch.testing.assert_close(lpz[rows].double(), ref, rtol=1e-5, atol=2e-5)
     torch.testing.assert_close(lpz, lp, rtol=2e-5, atol=2e-5)
     lp_b = ops.logprob(x, mu, sg, 1, B=B, HW=HW, math="tc")
@@ -500,7 +504,7 @@ def test_logprob_tc_bphw_tma_path():
     """[B,P,HW] written by 3-D TMA stores (taken when 32 | HW): against the exact fp32 kernel."""
     from mgproto_b200 import ops, _lib
     if not _lib.load().mgp_has_tensor_core_path():
-        pytest.skip("library built without the tcgen05 path")
+        pytest.skip("library built without the tensor-core path")
     B, HW, P, D = 5, 64, 300, 128
     g = torch.Generator().manual_seed(3)
     x = F.normalize(torch.randn(B * HW, D, generator=g), dim=1).to(_dev())
@@ -518,7 +522,7 @@ def test_push_search_from_the_top1_epilogue_vs_materialised_map():
     import mgproto_b200 as M
     from mgproto_b200 import ops, _lib
     if not _lib.load().mgp_has_tensor_core_path():
-        pytest.skip("library built without the tcgen05 path")
+        pytest.skip("library built without the tensor-core path")
     C, K, D, H, W, B = 12, 10, 128, 14, 14, 6
     torch.manual_seed(9)
     net = M.MGProto(features=nn.Sequential(nn.Conv2d(3, 16, 1)), img_size=H, prototype_shape=(C * K, D, 1, 1),
@@ -560,14 +564,21 @@ def test_push_prototypes_matches_oracle():
     labs = torch.randint(0, C, (n,), generator=g)
     labs[:C] = torch.arange(C)
     loader = [(imgs[i:i + 6], labs[i:i + 6]) for i in range(0, n, 6)]
-    with torch.no_grad():
-        feat, dist = net.push_forward(imgs.to(_dev()))
+    # the backbone runs at two batch sizes below (23 and 6): cuDNN's TF32 convolutions would make the copied features
+    # depend on the batch size's algorithm choice, so the comparison runs the convolutions in full fp32
+    tf32 = torch.backends.cudnn.allow_tf32
+    torch.backends.cudnn.allow_tf32 = False
+    try:
+        with torch.no_grad():
+            feat, dist = net.push_forward(imgs.to(_dev()))
+        mu0 = net.prototype_means.detach().clone()
+        res = M.push_prototypes(loader, net, log=lambda *_: None)
+    finally:
+        torch.backends.cudnn.allow_tf32 = tf32
     dist = dist.cpu().numpy()
     feat = feat.cpu().numpy()
     oi, ov = O.push_argmin(dist, labs.numpy(), K)
     want = O.push_assign(ov, labs.numpy(), C, K)
-    mu0 = net.prototype_means.detach().clone()
-    res = M.push_prototypes(loader, net, log=lambda *_: None)
     np.testing.assert_array_equal(res["image"], want)
     for j in range(C * K):
         c, k = divmod(j, K)

@@ -13,7 +13,7 @@ sys.path.insert(0, ROOT)
 from mgproto_b200 import ops  # noqa: E402
 
 peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(
-    os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6650.0
+    os.path.join(ROOT, "MEASURED_PEAKS.json")) else 3350.0
 dev = torch.device("cuda:0")
 B, HW, C = 256, 196, 200
 N = B * HW
@@ -27,7 +27,7 @@ for D in (64, 128, 256, 512):
         mu = F.normalize(torch.rand(P, D, generator=g), dim=1).to(dev)
         sg = torch.full((P, D), 0.3989422804, device=dev)
         out = torch.empty(N, P, device=dev)
-        path = "tcgen05 fp16x3" if D in (64, 128, 256) else "fp32 SIMT"
+        path = "wgmma fp16x3" if D in (64, 128, 256) else "fp32 SIMT"
         for _ in range(3):
             ops.logprob(x, mu, sg, 0, math="auto", out=out)
         torch.cuda.synchronize()

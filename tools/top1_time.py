@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Time the labelled step's max / arg-max log-likelihood kernel (logprob_tc_kernel<top1>, cfg2) with the ablation
-switches of MGP_TC_DEBUG: 1 no global results, 2 no TMEM loads, 4 no MMAs, 8 no epilogue work, 16 no prototype loads."""
+switches of MGP_TC_DEBUG: 1 no global results, 4 no MMAs, 8 no epilogue work, 16 no prototype loads."""
 import os
 import sys
 
