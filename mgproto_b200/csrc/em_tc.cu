@@ -17,16 +17,21 @@
 // classes' steps) is fp32 SIMT on the class's state, which stays in registers / shared memory for the whole timeline
 // exactly as in em_fused_kernel (em.cu); thread d owns mean / moment elements (k, d) for all k.
 //
-// Warpgroup 0 (warps 0-3) runs the E-step of a 128-row tile (two m64 halves: m64n32 with the X hi rows against
-// [means hi ; means lo], m64n16 with the X lo rows against means hi) and its soft-max straight from the accumulator
-// fragments (the 16 components of a row sit in 4 lanes).  Warpgroup 1 (warps 4-7) runs the statistics GEMM of the
-// tile (D / 64 m64 blocks) and keeps S1 in its registers across the tiles of a loop; at the end of a loop it hands
-// S1 to the owners through shared memory.  Two variants of the same kernel (template flag PIPE):
-//   * serial (D = 256; D = 128 when more classes are active than there are SMs): one tile buffer, the statistics
-//     of a tile follow its soft-max;
-//   * pipelined (D = 128, one CTA per SM, classes in the planner's order): three tile buffers and two R buffers; the
-//     TMA load of tile t+1 and the statistics of tile t-1 run under the E-step and soft-max of tile t.
-// Both are enqueued and the planner's count of active classes decides on the device which one does the work.
+// The E-step of a row tile (per m64 half: m64n32 with the X hi rows against [means hi ; means lo], m64n16 with the
+// X lo rows against means hi) is followed by its soft-max straight from the accumulator fragments (the 16 components
+// of a row sit in 4 lanes) and the statistics GEMM of the tile (D / 64 m64 blocks), which keeps S1 in registers across
+// the tiles of a loop; at the end of a loop S1 goes to the owners through shared memory.  Three variants of the same
+// kernel (template flag PIPE, and D):
+//   * serial, D = 256: two warpgroups, 128-row tiles, one tile buffer.  Warpgroup 0 (warps 0-3) runs the E-step and
+//     soft-max, then warpgroup 1 (warps 4-7) the statistics of the tile;
+//   * serial, D = 128 (more classes active than there are SMs): ONE warpgroup of 128 threads runs E-step, soft-max and
+//     statistics of a tile in turn (the two warpgroups above never overlap anyway), so that two CTAs share an SM and
+//     up to 2 x #SMs classes run in one wave.  64-row tiles -- tile t is the half t % 2 of a 128-row tile, so the MMAs
+//     into S1 come in the same order -- stream through a two-slot ring: the TMA load of tile t+1 runs under tile t;
+//   * pipelined (D = 128, one CTA per SM, classes in the planner's order): two warpgroups as in the first variant,
+//     three tile buffers and two R buffers; the TMA load of tile t+1 and the statistics of tile t-1 run under the
+//     E-step and soft-max of tile t.
+// At D = 128 both are enqueued and the planner's count of active classes decides on the device which one does the work.
 // HBM/L2 traffic: num_em_loop x (4 D + 4) bytes per bank row -- the algorithmic bytes of SURVEY 8(d) K-D.
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -41,8 +46,13 @@ using namespace mgp_tc;
 
 constexpr float SX = 256.0f;      // shadow rows hold 256 x (fp16 hi + lo)
 constexpr float SR = 1024.0f;     // responsibilities are stored as 1024 r
-constexpr int TR = 128;           // bank rows per tile (M of the E-step, K extent of the statistics GEMM)
 constexpr int S1_STRIDE = 17;     // S1 hand-over [D][17] fp32 (padded against bank conflicts)
+
+// the serial kernel at D = 128 is the one-warpgroup variant (two CTAs per SM, 64-row tiles); the others have two
+// warpgroups and 128-row tiles (bank rows per tile = M of the E-step, K extent of the statistics GEMM)
+__host__ __device__ constexpr bool em_one_wg(int D, bool pipe) { return !pipe && D == 128; }
+__host__ __device__ constexpr int em_threads(int D, bool pipe) { return em_one_wg(D, pipe) ? 128 : 256; }
+__host__ __device__ constexpr int em_rows(int D, bool pipe) { return em_one_wg(D, pipe) ? 64 : 128; }
 
 struct EmTcParams {
     const float* xx;              // [C*cap] |x|^2 of the bank rows (shadow)
@@ -86,29 +96,36 @@ __device__ __forceinline__ void warp_multi_reduce(float (&a)[V], int lane) {
 }
 
 template <int D, int KT, bool PIPE>
-__global__ void __launch_bounds__(256, 1)
+__global__ void __launch_bounds__(em_threads(D, PIPE), em_one_wg(D, PIPE) ? 2 : 1)
 em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_l, const EmTcParams prm) {
+    constexpr bool WG1 = em_one_wg(D, PIPE);       // one warpgroup runs everything (serial, D = 128)
+    constexpr int NT = em_threads(D, PIPE), NW = NT / 32;
+    constexpr int TR = em_rows(D, PIPE);           // bank rows per tile
     constexpr int NCH = D / 64;                    // 64-element (128 B) chunks along d
-    constexpr uint32_t CH_BYTES = TR * 128;        // one [128 rows x 64] fp16 block
+    constexpr uint32_t CH_BYTES = TR * 128;        // one [TR rows x 64] fp16 block
     constexpr uint32_t X_BYTES = NCH * CH_BYTES;   // hi (lo follows)
+    constexpr uint32_t R_BYTES = (TR / 64) * 4096; // one R buffer
     constexpr int OWN = D;                         // threads owning mean/moment elements: thread d <-> (k, d) for all k
     constexpr int MB = D / 64;                     // m64 blocks of the statistics GEMM
-    constexpr int ISSUER = 128;                    // the TMA issuing thread: lane 0 of warp 4 (warps 0-3 run the E-step)
+    constexpr int SW0 = NW - 4;                    // first warp of the warpgroup that runs the statistics GEMM
+    // the TMA issuing thread: lane 0 of warp 4 (warps 0-3 run the E-step), or thread 0 of the single warpgroup
+    constexpr int ISSUER = 32 * SW0;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
     uint8_t* bp = smem_raw + (base - raw);
     // carve-up (bytes from `base`)
-    constexpr int NXBUF = PIPE ? 3 : 1, NRBUF = PIPE ? 2 : 1;
+    constexpr int NXBUF = PIPE ? 3 : (WG1 ? 2 : 1), NRBUF = PIPE ? 2 : 1;
     const uint32_t o_xh = 0, o_xl = X_BYTES;                               // buffer b: + b * 2 * X_BYTES
     // means operand A and responsibilities R: per 64-wide K chunk one [32 rows x 128 B] block, rows 0-15 = hi,
     // rows 16-31 = lo, so ONE N = 32 MMA multiplies the row tile's hi half with both and an N = 16 MMA adds lo x hi
     const uint32_t o_a = NXBUF * 2 * X_BYTES;                             // [NCH][32][128 B]
-    const uint32_t o_r = o_a + NCH * 4096;                                // NRBUF x [2 (64-row chunks)][32][128 B]
+    const uint32_t o_r = o_a + NCH * 4096;                                // NRBUF x [TR / 64 (64-row chunks)][32][128 B]
     // S1 hand-over [D][S1_STRIDE]: its own region (!PIPE) or, PIPE, the tile buffer that is idle at the end of a loop
-    const uint32_t o_s1 = o_r + NRBUF * 8192;
+    const uint32_t o_s1 = o_r + NRBUF * R_BYTES;
     const uint32_t o_misc = o_s1 + (PIPE ? 0u : (uint32_t)((D * S1_STRIDE * 4 + 15) & ~15));
-    uint64_t* bars = reinterpret_cast<uint64_t*>(bp + o_misc);            // !PIPE: tma, (unused), stats | PIPE: xfull[3] xfree[3] (unused)[2] rfull[2]
+    // serial: tma, (unused), stats | one warpgroup: xfull[2] | PIPE: xfull[3] xfree[3] (unused)[2] rfull[2]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(bp + o_misc);
     float* s_e = reinterpret_cast<float*>(bars + 12);                     // [KT][KT]
     float* s_red = s_e + KT * KT;                                         // [8] + [8][16]
     float* s_w = s_red + 136;                                             // [16] w_k
@@ -276,8 +293,8 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
         return;
     }
     // the two replays' block-wide sums depend on the plan only: two otherwise idle warps evaluate them under the set-up
-    if (warp == 7) replay_prepare(step0, L * ord, s_misc);
-    if (warp == 6) replay_prepare(step0 + L * (ord + 1), L * (n_active - ord - 1), s_misc + 4);
+    if (warp == NW - 1) replay_prepare(step0, L * ord, s_misc);
+    if (warp == NW - 2) replay_prepare(step0 + L * (ord + 1), L * (n_active - ord - 1), s_misc + 4);
 
     if (tid == 0) MGP_PROF(63, 1);
     // ---- set-up: barriers, sigma-derived constants, zeroed operand tiles
@@ -285,6 +302,8 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
         if (PIPE) {                                  // xfree / rfull: one arrive per warp of the consuming warpgroup
             for (int i = 0; i < 3; ++i) { mbar_init(bar_tma + 8u * i, 1); mbar_init(bar_tma + 8u * (3 + i), 4); }
             for (int i = 0; i < 2; ++i) mbar_init(bar_tma + 8u * (8 + i), 4);
+        } else if (WG1) {
+            for (int i = 0; i < 2; ++i) mbar_init(bar_tma + 8u * i, 1);
         } else {
             mbar_init(bar_tma, 1);
             mbar_init(bar_s, 4);
@@ -292,10 +311,10 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     bool same = true;
-    for (int i = tid; i < KD; i += 256) same = same && (sg_c[i] == sg_c[(i / D) * D]);
-    for (uint32_t i = tid * 16u; i < NCH * 4096u + NRBUF * 8192u; i += 256u * 16u)     // A and R blocks: rows >= K stay zero
+    for (int i = tid; i < KD; i += NT) same = same && (sg_c[i] == sg_c[(i / D) * D]);
+    for (uint32_t i = tid * 16u; i < NCH * 4096u + NRBUF * R_BYTES; i += NT * 16u)     // A and R blocks: rows >= K stay zero
         *reinterpret_cast<uint4*>(bp + o_a + i) = make_uint4(0u, 0u, 0u, 0u);
-    for (int i = tid; i < KT * KT; i += 256) s_e[i] = 0.f;
+    for (int i = tid; i < KT * KT; i += NT) s_e[i] = 0.f;
     if (tid < 16) {
         float w = 0.f, ls = 0.f, pi = 0.f;
         if (tid < K) {
@@ -321,7 +340,7 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
     const float div_scale = -4.0f * prm.lamda / ((float)K * (float)(K - 1));
     uint32_t tile_ctr = 0;                                           // tiles issued so far (mbarrier phases)
     const int t4 = lane & 3, g8 = lane >> 2;                         // accumulator fragment coordinates (tc_ptx.cuh)
-    float s32[MB][16], s16[MB][8];                                   // warpgroup 1: S1 of the current loop
+    float s32[MB][16], s16[MB][8];                                   // statistics warpgroup: S1 of the current loop
 #pragma unroll
     for (int mb = 0; mb < MB; ++mb) {
 #pragma unroll
@@ -330,14 +349,15 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
         for (int j = 0; j < 8; ++j) s16[mb][j] = 0.f;
     }
 
-    // E-step of one tile + soft-max + R (warpgroup 0).  E-step: A = X (K-major), B = [means hi ; means lo] (K-major):
-    // N = 32 with X hi, N = 16 (means hi only) with X lo; rows h * 64 + 16 warp + g8 + 8 rr of the tile, components
-    // k = 8 i + 2 t4 + j (columns k: hi.hi, 16 + k: hi.lo; the N = 16 accumulator: lo.hi).
+    // E-step of one tile + soft-max + R (warps 0-3).  E-step: A = X (K-major), B = [means hi ; means lo] (K-major):
+    // N = 32 with X hi, N = 16 (means hi only) with X lo; rows h * 64 + 16 warp + g8 + 8 rr of the tile (NH m64
+    // halves), components k = 8 i + 2 t4 + j (columns k: hi.hi, 16 + k: hi.lo; the N = 16 accumulator: lo.hi).
     // before_write() runs between the soft-max and the R stores (PIPE: wait until the R buffer is free)
+    constexpr int NH = TR / 64;
     auto estep_tile = [&](uint32_t xb, uint8_t* rbp, int t, float inv_a, float (&s0v)[4], auto&& before_write) {
-        float e32[2][16], e16[2][8];
+        float e32[NH][16], e16[NH][8];
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
+        for (int h = 0; h < NH; ++h) {
 #pragma unroll
             for (int j = 0; j < 16; ++j) e32[h][j] = 0.f;
 #pragma unroll
@@ -349,16 +369,16 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
             const uint32_t xo = (uint32_t)(ks >> 2) * CH_BYTES + (uint32_t)(ks & 3) * 32u;
             const uint64_t bd = gmma_desc(base + o_a + (uint32_t)(ks >> 2) * 4096u + (uint32_t)(ks & 3) * 32u);
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {                            // rows 64 h .. 64 h + 63 of the tile: + 8 KiB
+            for (int h = 0; h < NH; ++h) {                           // rows 64 h .. 64 h + 63 of the tile: + 8 KiB
                 wg_mma_n32<0>(e32[h], gmma_desc(xb + o_xh + xo + (uint32_t)h * 8192u), bd, 1u);
                 wg_mma_n16<0>(e16[h], gmma_desc(xb + o_xl + xo + (uint32_t)h * 8192u), bd, 1u);
             }
         }
         wg_commit();
         wg_wait0();
-        float rr_v[2][2][4];
+        float rr_v[NH][2][4];
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
+        for (int h = 0; h < NH; ++h)
 #pragma unroll
             for (int rr = 0; rr < 2; ++rr) {
                 const int row = t * TR + h * 64 + 16 * warp + g8 + 8 * rr;
@@ -392,7 +412,7 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
             }
         before_write();
 #pragma unroll
-            for (int h = 0; h < 2; ++h)
+            for (int h = 0; h < NH; ++h)
 #pragma unroll
                 for (int rr = 0; rr < 2; ++rr) {
                     const int rt = h * 64 + 16 * warp + g8 + 8 * rr;     // row within the tile
@@ -414,7 +434,7 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
                 }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // R stores -> visible to the MMA (async proxy)
     };
-    // statistics of one tile (warpgroup 1): S1 += X^T . [R hi ; R lo] (m64n32, A = X hi MN-major) and X lo^T . R hi
+    // statistics of one tile (warps SW0 .. SW0 + 3): S1 += X^T . [R hi ; R lo] (m64n32, A = X hi MN-major) and X lo^T . R hi
     // (m64n16), one m64 block per 64 d
     auto stats_tile = [&](uint32_t xb, uint32_t rb, bool first) {
         wg_fence();
@@ -433,7 +453,7 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
         wg_wait0();
     };
 
-    auto load_tile = [&](int t) {                                    // issuer only: one 128-row tile, hi + lo, into the X buffer
+    auto load_tile = [&](int t) {                                    // issuer only (serial, D = 256): one tile, hi + lo, into the X buffer
         mbar_expect_tx(bar_tma, 2 * X_BYTES);
         const int row0 = c * cap + t * TR;
 #pragma unroll
@@ -491,7 +511,7 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
         {
             float mx = 0.f;
 #pragma unroll
-            for (int w8 = 0; w8 < 8; ++w8) mx = fmaxf(mx, s_red[w8]);
+            for (int w8 = 0; w8 < NW; ++w8) mx = fmaxf(mx, s_red[w8]);
             int ex = 0;
             if (mx > 0.f) frexpf(mx, &ex);
             a_scale = ldexpf(1.0f, 8 - ex);                          // max |a| * scale in [128, 256)
@@ -502,8 +522,9 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
             for (int w8 = 0; w8 < OWN / 32; ++w8) mm += s_pair[w8 * PV + NPAIR + tid];
             s_cst[tid] = -s_ls[tid] + logf(s_pi[tid] + EM_EPS) - 0.5f * s_w[tid] * mm;   // ref :316, :323-336
         }
-        if (tid >= 32 && tid < 32 + NPAIR) {                         // exp(-|mu_i - mu_j|^2), ref model.py:390-392
-            const int pr = tid - 32;
+        // exp(-|mu_i - mu_j|^2), ref model.py:390-392: pair pr on thread 32 + pr (one warpgroup: (32 + pr) % 128)
+        static_assert(NPAIR <= 128, "one thread per pair");
+        if (const int pr = WG1 ? (tid + NT - 32) % NT : tid - 32; pr >= 0 && pr < NPAIR) {
             int i = 0, rem = pr;
             while (rem >= KT - 1 - i) { rem -= KT - 1 - i; ++i; }
             const int j = i + 1 + rem;
@@ -527,7 +548,7 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // operand stores -> visible to the MMA (async proxy)
         __syncthreads();
 
-        float s0v[4] = {0.f, 0.f, 0.f, 0.f};                          // warpgroup 0: S0 of components 8 (q / 2) + 2 t4 + q % 2
+        float s0v[4] = {0.f, 0.f, 0.f, 0.f};                          // warps 0-3: S0 of components 8 (q / 2) + 2 t4 + q % 2
         const float inv_a = 1.0f / (a_scale * SX);
         uint32_t s1_base;                                             // the S1 hand-over of this loop
 
@@ -586,6 +607,40 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
             }
             tile_ctr += (uint32_t)ntiles;
             s1_base = base + ((tile_ctr + 1u) % 3u) * 2 * X_BYTES;   // idle until the next loop's second tile
+        } else if constexpr (WG1) {
+            // xfull[s]: a tile landed in slot s.  Tile g of the class's timeline (row tile g % ntiles of loop
+            // g / ntiles) goes to slot g & 1, so xfull[s] completes once per tile in slot s: phase parity (g / 2) & 1.
+            // Slot g & 1 takes tile g + 2 as soon as the statistics MMAs of tile g have retired.
+            const uint32_t n_total = (uint32_t)(L * ntiles);
+            auto xslot = [&](uint32_t g) { return base + (g & 1u) * 2 * X_BYTES; };
+            auto load_tile_r = [&](uint32_t g) {                     // issuer only
+                const uint32_t bar = bar_tma + 8u * (g & 1u);
+                mbar_expect_tx(bar, 2 * X_BYTES);
+                const int row0 = c * cap + (int)(g % (uint32_t)ntiles) * TR;
+#pragma unroll
+                for (int ch = 0; ch < NCH; ++ch) {
+                    tma_load_2d(xslot(g) + o_xh + ch * CH_BYTES, &map_h, ch * 64, row0, bar);
+                    tma_load_2d(xslot(g) + o_xl + ch * CH_BYTES, &map_l, ch * 64, row0, bar);
+                }
+                MGP_PROF(g, 0);
+            };
+            if (tid == ISSUER && loop == 0) {
+                load_tile_r(0);
+                if (n_total > 1) load_tile_r(1);
+            }
+            for (int t = 0; t < ntiles; ++t, ++tile_ctr) {
+                const uint32_t g = tile_ctr;
+                mbar_wait(bar_tma + 8u * (g & 1u), (g >> 1) & 1u);
+                if (tid == 0) MGP_PROF(g, 1);
+                estep_tile(xslot(g), bp + o_r, t, inv_a, s0v, []() {});
+                if (tid == 0) MGP_PROF(g, 4);
+                __syncthreads();                                     // every warp's R rows are stored and fenced
+                stats_tile(xslot(g), base + o_r, t == 0);
+                if (tid == 0) MGP_PROF(g, 5);
+                __syncthreads();                                     // every warp's statistics MMAs retired: slot and R free
+                if (tid == ISSUER && g + 2 < n_total) load_tile_r(g + 2);   // (a loop's last two: the next loop's first two)
+            }
+            s1_base = base + o_s1;
         } else {
         for (int t = 0; t < ntiles; ++t, ++tile_ctr) {
             const uint32_t par = tile_ctr & 1u;
@@ -619,7 +674,7 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
         s1_base = base + o_s1;
         }   // !PIPE
         if (tid == 0) MGP_PROF(tile_ctr - 1, 6);
-        // ---- S0 over the class (warpgroup 0: reduce over the 8 rows of a fragment column, then lanes 0-3 hold all 16)
+        // ---- S0 over the class (warps 0-3: reduce over the 8 rows of a fragment column, then lanes 0-3 hold all 16)
         if (warp < 4) {
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
@@ -630,16 +685,16 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
                 if (g8 == 0) s_red[warp * 16 + 8 * (q >> 1) + 2 * t4 + (q & 1)] = v;
             }
         }
-        // ---- S1 from warpgroup 1's registers to the owners: s1[d][k] = (hi.hi + lo.hi) + hi.lo
+        // ---- S1 from the statistics warpgroup's registers to the owners: s1[d][k] = (hi.hi + lo.hi) + hi.lo
         float* s_s1 = reinterpret_cast<float*>(bp + (s1_base - base));
-        if (warp >= 4) {
+        if (warp >= SW0) {
 #pragma unroll
             for (int mb = 0; mb < MB; ++mb)
 #pragma unroll
                 for (int rr = 0; rr < 2; ++rr)
 #pragma unroll
                     for (int q = 0; q < 4; ++q) {
-                        const int d = mb * 64 + 16 * (warp - 4) + g8 + 8 * rr, k = 8 * (q >> 1) + 2 * t4 + (q & 1);
+                        const int d = mb * 64 + 16 * (warp - SW0) + g8 + 8 * rr, k = 8 * (q >> 1) + 2 * t4 + (q & 1);
                         const int idx = 4 * (q >> 1) + 2 * rr + (q & 1);
                         s_s1[d * S1_STRIDE + k] = (s32[mb][idx] + s16[mb][idx]) + s32[mb][idx + 8];
                     }
@@ -698,7 +753,8 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
 
 template <int D>
 size_t em_tc_smem(int kt, bool pipe) {
-    return 1024 + (pipe ? 3 : 1) * 2 * (size_t)(D / 64) * TR * 128 + (size_t)(D / 64) * 4096 + (pipe ? 2 : 1) * 8192 +
+    const size_t tr = em_rows(D, pipe), nx = pipe ? 3 : (em_one_wg(D, pipe) ? 2 : 1);
+    return 1024 + nx * 2 * (size_t)(D / 64) * tr * 128 + (size_t)(D / 64) * 4096 + (pipe ? 2 : 1) * (tr / 64) * 4096 +
            (pipe ? 0 : (size_t)((D * S1_STRIDE * 4 + 15) & ~15)) +
            ((size_t)kt * kt + 136 + 6 * 16 + 8 + 8 * (size_t)(32 * ((kt * (kt - 1) / 2 + kt + 31) / 32))) * 4 + 128;
 }
@@ -718,9 +774,11 @@ int mgp_em_tc_launch(const void* shadow_h, const void* shadow_l, const float* sh
                      const int32_t* sched, float* mu, const float* sigma, float* weight, float* exp_avg, float* exp_avg_sq,
                      int* status, int num_em_loop, float alpha, double lr, double beta1, double beta2, double adam_eps,
                      double tau, float lamda, int C, int K, int D, int cap, cudaStream_t st) {
-    CUtensorMap mh, ml;
+    CUtensorMap mh, ml, mh1, ml1;                   // 128-row boxes; 64-row boxes for the one-warpgroup kernel (D = 128)
     const uint64_t rows = (uint64_t)C * cap;
-    if (!make_map_f16(&mh, shadow_h, rows, D, TR) || !make_map_f16(&ml, shadow_l, rows, D, TR)) return MGP_ERR_UNSUPPORTED;
+    if (!make_map_f16(&mh, shadow_h, rows, D, 128) || !make_map_f16(&ml, shadow_l, rows, D, 128)) return MGP_ERR_UNSUPPORTED;
+    if (D == 128 && (!make_map_f16(&mh1, shadow_h, rows, D, 64) || !make_map_f16(&ml1, shadow_l, rows, D, 64)))
+        return MGP_ERR_UNSUPPORTED;
     EmTcParams prm;
     prm.xx = shadow_xx; prm.bc = bias_corr; prm.order = order; prm.sched = sched; prm.mu = mu; prm.sigma = sigma; prm.weight = weight;
     prm.exp_avg = exp_avg; prm.exp_avg_sq = exp_avg_sq; prm.status = status;
@@ -737,24 +795,24 @@ int mgp_em_tc_launch(const void* shadow_h, const void* shadow_l, const float* sh
         MGP_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, devi));
     }
     prm.pipe_max = pipe ? n_sm : 0;
-#define MGP_EMTC(DD, KK, PP)                                                                                        \
+#define MGP_EMTC(DD, KK, PP, MH, ML)                                                                                \
     do {                                                                                                            \
         const size_t smem = em_tc_smem<DD>(KK, PP);                                                                 \
         MGP_CUDA(cudaFuncSetAttribute(em_tc_kernel<DD, KK, PP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        em_tc_kernel<DD, KK, PP><<<C, 256, smem, st>>>(mh, ml, prm);                                                \
+        em_tc_kernel<DD, KK, PP><<<C, em_threads(DD, PP), smem, st>>>(MH, ML, prm);                                 \
     } while (0)
-#define MGP_EMTC_K(DD, PP)                                                                                          \
+#define MGP_EMTC_K(DD, PP, MH, ML)                                                                                  \
     do {                                                                                                            \
-        if (K <= 5) MGP_EMTC(DD, 5, PP);                                                                            \
-        else if (K <= 10) MGP_EMTC(DD, 10, PP);                                                                     \
-        else MGP_EMTC(DD, 16, PP);                                                                                  \
+        if (K <= 5) MGP_EMTC(DD, 5, PP, MH, ML);                                                                    \
+        else if (K <= 10) MGP_EMTC(DD, 10, PP, MH, ML);                                                             \
+        else MGP_EMTC(DD, 16, PP, MH, ML);                                                                          \
     } while (0)
     if (D == 128) {
-        if (pipe) MGP_EMTC_K(128, true);
+        if (pipe) MGP_EMTC_K(128, true, mh, ml);
         MGP_CHECK_LAUNCH();
-        MGP_EMTC_K(128, false);                      // (returns at once when the pipelined kernel took the call)
+        MGP_EMTC_K(128, false, mh1, ml1);            // one warpgroup (returns at once when the pipelined kernel took the call)
     } else {
-        MGP_EMTC_K(256, false);
+        MGP_EMTC_K(256, false, mh, ml);
     }
 #undef MGP_EMTC_K
 #undef MGP_EMTC

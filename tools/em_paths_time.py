@@ -1,7 +1,10 @@
 #!/usr/bin/env python
-"""Time update_GMM (all classes active, cfg2 / cfg3 mixture shapes) through each implementation: tensor-core kernel,
-fp32 cluster kernel, multi-launch path.  CUDA events, 20 calls after 3 warm-ups."""
+"""Time update_GMM (cfg2 / cfg3 mixture shapes) through each implementation: tensor-core kernel, fp32 cluster kernel,
+multi-launch path, at 80 .. 200 active classes.  At D = 128 the tensor-core kernel takes its pipelined variant while
+the active classes fit one CTA per SM (132 on an H100 SXM) and its one-warpgroup variant (two CTAs per SM) beyond;
+tc_serial always takes the latter.  CUDA events, 20 calls after 3 warm-ups; prints the card and its power limit."""
 import os
+import subprocess
 import sys
 
 import torch
@@ -14,6 +17,9 @@ from mgproto_b200 import _lib                  # noqa: E402
 dev = torch.device("cuda:0")
 torch.cuda.set_device(0)
 lib = _lib.load()
+card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
+                      stdout=subprocess.PIPE, text=True).stdout.strip()
+print("card: %s, %d SMs" % (card, torch.cuda.get_device_properties(0).multi_processor_count))
 for D in (128, 256):
     bench.CFG["D"] = D
     net = bench.build_model(dev)
@@ -24,7 +30,7 @@ for D in (128, 256):
         lib.mgp_set_option(b"em_tc", tc)
         lib.mgp_set_option(b"em_fused", fused)
         lib.mgp_set_option(b"em_pipe", pipe)
-        for n_act in (200, 146, 100):
+        for n_act in (80, 132, 133, 146, 200):
             def run():
                 net.queue.updated.zero_()
                 net.queue.updated[:n_act] = 1
