@@ -23,6 +23,13 @@
 //            consecutive floats of one output row), affine fix-up, stores.
 // HBM traffic per launch: 4*N*P (output) + 8*N*Kg (fp16 hi/lo operand written by the prep pass and
 // read once) + 4*N*D (x) -- the output dominates; the kernel is bound by the HBM write stream.
+//
+// The labelled step's per (image, prototype) max / arg-max (MGP_OUT_TOP1_BP) with isotropic sigma, 32 <= HW <= 256 and
+// D in {64, 128} takes logprob_top1_wide_kernel instead: one x tile per image, one m64nNIk16 MMA per k16 step and pass
+// (NI = HW rounded up to 32, 56, 64, 128, 200 or 256), the max / arg-max read straight from the accumulator fragments and
+// written with plain stores; nothing is stored but B*P packed results, so it is bound by the tensor cores.  Its other
+// cases (anisotropic sigma, other HW, D = 256) run logprob_tc_kernel<top1> on 128-patch tiles, into a zeroed output
+// by 64-bit RED.MAX.
 #include <cuda.h>
 #include <cstdlib>
 #include <cuda_fp16.h>
@@ -149,6 +156,7 @@ struct TcParams {
                            // adjacent prototype tiles, so each output row receives team*512 contiguous bytes at once
     uint32_t smem_bytes;   // dynamic shared memory of the launch
     int x_no_sq;           // the staged patch operands lack the x^2 half (isotropic sigma asserted by the producer)
+    int iso_elsewhere;     // top-1 fallback: return at once when sigma turns out isotropic (the image-tile kernel ran)
     int debug;   // ablation switches for profiling (MGP_TC_DEBUG): 1 no global stores, 4 no MMAs,
                  // 8 no epilogue work, 16 no prototype TMA loads
 };
@@ -159,8 +167,7 @@ template <int LAYOUT>
 __device__ __forceinline__ void epilogue_chunk(const uint32_t (&r)[32], const float* __restrict__ s_sn_c, float c0,
                                                float c1, float c2, int n0, int p, bool pok, const TcParams& prm,
                                                float* stg = nullptr, const CUtensorMap* map_out = nullptr, int img_b = 0,
-                                               int img_hw0 = 0, bool img = false, float* run_v = nullptr,
-                                               int* run_i = nullptr) {
+                                               int img_hw0 = 0) {
     const int N = prm.N, P = prm.P, HW = prm.HW;
     float v[32];
     const float4* s4 = reinterpret_cast<const float4*>(s_sn_c);    // |x_n|^2 of the 32 columns (shared memory)
@@ -178,33 +185,9 @@ __device__ __forceinline__ void epilogue_chunk(const uint32_t (&r)[32], const fl
     if (LAYOUT == LAYOUT_TOP1) {
         // only max_n log p[n, p] and its patch per image are wanted (labelled training step: the reference aliases
         // the other levels of wrong-class prototypes to level 0): nothing is stored, the log-likelihood matrix
-        // never reaches HBM.  Image tiles keep a running (max, patch) across the warp's chunks (the caller issues
-        // one 64-bit RED.MAX per tile); 128-patch tiles may cross image ends and reduce per image segment.
-        if (img) {
-            // chunk maximum by a tree of FMNMX (one instruction per column); the position is only looked up when the
-            // chunk beats the running maximum (a few times per image): same result as the strict left-to-right scan
-            // (first patch wins ties) at ~2 instead of ~5 instructions per column
-            if (img_hw0 + 32 > HW) {                              // the image's last chunk: columns beyond HW do not exist
-#pragma unroll
-                for (int j = 0; j < 32; ++j)
-                    if (img_hw0 + j >= HW) v[j] = -INFINITY;
-            }
-            float m[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) m[j] = fmaxf(v[2 * j], v[2 * j + 1]);
-#pragma unroll
-            for (int w = 8; w >= 1; w >>= 1)
-#pragma unroll
-                for (int j = 0; j < w; ++j) m[j] = fmaxf(m[j], m[j + w]);
-            if (m[0] > *run_v) {
-                int idx = 31;
-#pragma unroll
-                for (int j = 30; j >= 0; --j) idx = (v[j] == m[0]) ? j : idx;
-                *run_v = m[0];
-                *run_i = img_hw0 + idx;
-            }
-            return;
-        }
+        // never reaches HBM.  This is the 128-patch-tile fallback (anisotropic sigma, HW outside [32, 256], D = 256;
+        // image tiles take logprob_top1_wide_kernel): a tile may cross image ends, so the chunk is reduced per image
+        // segment and merged by a 64-bit RED.MAX into the zeroed `best`.
         if (!pok) return;
         unsigned long long* best = reinterpret_cast<unsigned long long*>(prm.out);
         int b = n0 / HW, hw = n0 - b * HW;
@@ -312,7 +295,7 @@ logprob_tc_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_const
     constexpr bool TMA_ST = (LAYOUT == LAYOUT_NP_TMA || LAYOUT == LAYOUT_BPHW_TMA || LAYOUT == LAYOUT_NEGP_TMA);
     constexpr bool BPHW_TMA = (LAYOUT == LAYOUT_BPHW_TMA || LAYOUT == LAYOUT_NEGP_TMA);
     // image tiles (up to 256 patches = 8 chunks) exist only for these layouts; 128-patch tiles have 4 chunks
-    constexpr int NCH = (BPHW_TMA || LAYOUT == LAYOUT_TOP1) ? 8 : 4;
+    constexpr int NCH = BPHW_TMA ? 8 : 4;
     // the layout used by the non-TMA fallback of the same instantiation (anisotropic sigma: see `img` below)
     constexpr int STG_LAYOUT = (LAYOUT == LAYOUT_BPHW_TMA) ? MGP_OUT_LOGP_BPHW
                                : (LAYOUT == LAYOUT_NEGP_TMA) ? MGP_OUT_NEGP_BPHW : LAYOUT;
@@ -323,12 +306,13 @@ logprob_tc_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_const
 
     const bool gen = (*prm.noniso != 0);
     if (gen && (prm.D > 128 || prm.x_no_sq)) __trap();            // isotropic sigma was promised (MGP_MATH_TC_ISO / staging): fail loudly
+    if (LAYOUT == LAYOUT_TOP1 && prm.iso_elsewhere && !gen) return;   // isotropic: logprob_top1_wide_kernel has done the work
     const int nkb = (gen ? 2 * prm.D : prm.D) / KB;               // K blocks per tile
     const int kcol0 = gen ? 0 : prm.D;                            // isotropic: only the [x] / [-2 w mu] half
     // [B,P,HW] through TMA: one x tile = one image (nti = round_up(HW,32) patches) so that no 32-column chunk
     // crosses an image end.  The wider tile only fits when sigma is isotropic (K = D); otherwise this
     // instantiation falls back to 128-patch tiles and register stores.
-    const bool img = (BPHW_TMA || (LAYOUT == LAYOUT_TOP1 && prm.xbox == 32)) && !gen;
+    const bool img = BPHW_TMA && !gen;
     const int NT = img ? prm.nti : 128;                           // patches per tile
     const int nch = NT / 32;                                      // 32-patch MMA chunks (m64n32k16 each)
     const int row_step = img ? prm.HW : 128;                      // first patch row of x tile nt = nt * row_step
@@ -477,8 +461,6 @@ logprob_tc_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_const
                 const float c0 = pok ? __ldg(prm.e0 + p) : 0.f;
                 const float c1 = pok ? __ldg(prm.e1 + p) : 0.f;
                 const float c2 = (pok && !gen) ? __ldg(prm.e2 + p) : 0.f;
-                float run_v = -INFINITY;                          // LAYOUT_TOP1, image tiles: best of this thread's chunks
-                int run_i = -1;
 #pragma unroll
                 for (int pass = 0; pass < NCH / 2; ++pass) {
                     if (2 * pass >= nch) break;
@@ -511,17 +493,213 @@ logprob_tc_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_const
                     if (ch < nch) {
                         if (!BPHW_TMA || img)
                             epilogue_chunk<LAYOUT>(rv, s_sn + ch * 32, c0, c1, c2, row0 + ch * 32, p, pok, prm, stg, &map_out,
-                                                   nt, ch * 32, img, &run_v, &run_i);
+                                                   nt, ch * 32);
                         else
                             epilogue_chunk<STG_LAYOUT>(rv, s_sn + ch * 32, c0, c1, c2, row0 + ch * 32, p, pok, prm);
                     }
                 }
-                if (LAYOUT == LAYOUT_TOP1 && img && pok && run_i >= 0 && !(prm.debug & 1))
-                    atomicMax(reinterpret_cast<unsigned long long*>(prm.out) + (size_t)nt * prm.P + p,
-                              top1_pack(run_v, run_i));
             }
         }
         if (TMA_ST && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // stores landed
+    }
+}
+
+// ------------------------------------------------------------------------------------------ top-1, image tiles
+// Per (image, prototype) max / arg-max of log p for isotropic sigma, 32 <= HW <= 256, D in {64, 128}.  An x tile is
+// one image, NI = HW rounded up to the next instantiated width; columns >= HW belong to the next image (or lie past
+// N and read as zero) and are masked.  Same warp roles and team schedule as logprob_tc_kernel:
+//   warp 9   TMA producer of the x tile: one NI-row box per K block and hi / lo half, each K block with its own
+//            full / empty barrier pair, so the next image's first K block loads while the current image's last
+//            prototype tile still multiplies its second one
+//   warp 8   TMA producer of the prototype K blocks (128 rows) through an S-stage ring
+//   warps 0-7  warpgroup g multiplies prototype rows [64 g, 64 g + 64) of the tile with the whole image: per k16
+//            step one m64nNIk16 MMA per pass (hi*hi, lo*hi, hi*lo), one commit group per K block, the previous K
+//            block's group retired (and its stage released) while the current one runs.  The epilogue reads the
+//            fragments in place: a thread holds 2 prototype rows x NI / 4 columns; it keeps the running (max, first
+//            column) of each row, a quad of lanes merges its four by two shuffles, and lane 0 of the quad writes the
+//            packed result with a plain 64-bit store -- every (image, prototype) pair has exactly one writer, so
+//            `best` needs no zeroing and no atomics.
+// HW_MIN: the smallest HW this width serves; 8-column blocks below it need no mask.
+template <int NI, int HW_MIN>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+logprob_top1_wide_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_constant__ CUtensorMap map_xl,
+                         const __grid_constant__ CUtensorMap map_ph, const __grid_constant__ CUtensorMap map_pl,
+                         const TcParams prm) {
+    static_assert(NI % 8 == 0 && NI >= 32 && NI <= 256 && HW_MIN <= NI, "wgmma N");
+    constexpr int R = NI / 2;                                     // accumulator registers per thread
+    constexpr uint32_t XSUB = (uint32_t)NI * KB * 2;              // one [NI x 64] fp16 block of the x tile
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t raw = smem_u32(smem_raw);
+    const uint32_t base = (raw + 1023u) & ~1023u;                 // SWIZZLE_128B tiles need 1024 B alignment
+    uint8_t* base_ptr = smem_raw + (base - raw);
+
+    if (*prm.noniso != 0) {                                       // anisotropic: the 128-patch-tile kernel runs instead
+        if (!prm.iso_elsewhere) __trap();                         // ... unless isotropic sigma was promised: fail loudly
+        return;
+    }
+    const int nkb = prm.D / KB;                                   // 1 or 2 K blocks, the [x] / [-2 w mu] half only
+    const int kcol0 = prm.D;
+
+    // carve-up: nbuf x tiles (hi blocks then lo blocks) | S prototype stages | barriers | |x|^2 of two images
+    const uint32_t x_bytes = (uint32_t)(2 * nkb) * XSUB;
+    const uint32_t tile_budget = prm.smem_bytes - 1024u - 4096u;
+    const int nbuf = (2 * x_bytes + 4 * 2 * SUB_BYTES <= tile_budget) ? 2 : 1;   // double-buffer x when 4 stages still fit
+    int S = (int)((tile_budget - nbuf * x_bytes) / (2 * SUB_BYTES));
+    if (S > 6) S = 6;
+    const uint32_t x_base = base;
+    const uint32_t st_base = x_base + nbuf * x_bytes;
+    const uint32_t misc = st_base + (uint32_t)S * 2 * SUB_BYTES;
+    const uint32_t bar0 = misc;                                   // full[6] empty[6] xfull[2][2] xempty[2][2]
+    auto FULL = [&](int i) { return bar0 + 8u * i; };
+    auto EMPTY = [&](int i) { return bar0 + 8u * (6 + i); };
+    auto XFULL = [&](int b, int kb) { return bar0 + 8u * (12 + 2 * b + kb); };
+    auto XEMPTY = [&](int b, int kb) { return bar0 + 8u * (16 + 2 * b + kb); };
+    float* s_sn = reinterpret_cast<float*>(base_ptr + (misc - base) + 256);   // [2][256]
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) {
+        for (int i = 0; i < 6; ++i) { mbar_init(FULL(i), 1); mbar_init(EMPTY(i), 8); }   // empty: one arrive per consumer warp
+        for (int b = 0; b < 2; ++b)
+            for (int kb = 0; kb < 2; ++kb) { mbar_init(XFULL(b, kb), 1); mbar_init(XEMPTY(b, kb), 8); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    const int TS = prm.team;
+    const int n_teams = gridDim.x / TS, team = blockIdx.x / TS, k0 = blockIdx.x % TS;
+    const int n_ptiles = prm.n_ptiles, B = prm.B, HW = prm.HW;
+    if (team >= n_teams || k0 >= n_ptiles) return;                // nothing to do for this CTA (tiny problems)
+
+    if (warp == 9) {
+        // =========================== x-tile TMA producer ===========================
+        if (lane == 0) {
+            int c = 0;
+            for (int nt = team; nt < B; nt += n_teams, ++c) {
+                const int buf = c % nbuf, use = c / nbuf;
+                const uint32_t xb = x_base + (uint32_t)buf * x_bytes;
+                for (int kb = 0; kb < nkb; ++kb) {
+                    if (use > 0) mbar_wait(XEMPTY(buf, kb), (uint32_t)((use - 1) & 1));
+                    mbar_expect_tx(XFULL(buf, kb), 2 * XSUB);
+                    tma_load_2d(xb + (uint32_t)kb * XSUB, &map_xh, kcol0 + kb * KB, nt * HW, XFULL(buf, kb));
+                    tma_load_2d(xb + (uint32_t)(nkb + kb) * XSUB, &map_xl, kcol0 + kb * KB, nt * HW, XFULL(buf, kb));
+                }
+            }
+        }
+    } else if (warp == 8) {
+        // =========================== prototype TMA producer ===========================
+        if (lane == 0) {
+            int stage = 0;
+            uint32_t phase = 0;
+            for (int nt = team; nt < B; nt += n_teams)
+                for (int pt = k0; pt < n_ptiles; pt += TS)
+                    for (int kb = 0; kb < nkb; ++kb) {
+                        mbar_wait(EMPTY(stage), phase ^ 1u);
+                        if (prm.debug & 16) {
+                            mbar_arrive(FULL(stage));
+                        } else {
+                            mbar_expect_tx(FULL(stage), 2 * SUB_BYTES);
+                            const uint32_t dst = st_base + (uint32_t)stage * 2 * SUB_BYTES;
+                            tma_load_2d(dst, &map_ph, kcol0 + kb * KB, pt * PT, FULL(stage));
+                            tma_load_2d(dst + SUB_BYTES, &map_pl, kcol0 + kb * KB, pt * PT, FULL(stage));
+                        }
+                        if (++stage == S) { stage = 0; phase ^= 1u; }
+                    }
+        }
+    } else {
+        // =========================== consumers: MMA + epilogue ===========================
+        const int wg = warp >> 2, wq = warp & 3, q = lane & 3;
+        const int prow = wg * 64 + 16 * wq + (lane >> 2);         // this thread's prototype rows: prow and prow + 8
+        unsigned long long* best = reinterpret_cast<unsigned long long*>(prm.out);
+        int stage = 0, c = 0;
+        uint32_t phase = 0;
+        for (int nt = team; nt < B; nt += n_teams, ++c) {
+            const int buf = c % nbuf;
+            const uint32_t xpar = (uint32_t)((c / nbuf) & 1);
+            const uint32_t xb = x_base + (uint32_t)buf * x_bytes;
+            // |x|^2 of this image, double-buffered by image: the readers of buffer c & 1 (image c - 2) all passed
+            // the previous image's barrier
+            float* sn = s_sn + (c & 1) * 256;
+            for (int i = threadIdx.x; i < NI; i += 256) sn[i] = (i < HW) ? prm.sn[(size_t)nt * HW + i] : 0.f;
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+            for (int pt = k0; pt < n_ptiles; pt += TS) {
+                const bool last = pt + TS >= n_ptiles;            // last prototype tile of this image: release x
+                const int p0 = pt * PT + prow, p1 = p0 + 8;
+                const float c0a = p0 < prm.P ? __ldg(prm.e0 + p0) : 0.f, c0b = p1 < prm.P ? __ldg(prm.e0 + p1) : 0.f;
+                const float c1a = p0 < prm.P ? __ldg(prm.e1 + p0) : 0.f, c1b = p1 < prm.P ? __ldg(prm.e1 + p1) : 0.f;
+                const float c2a = p0 < prm.P ? __ldg(prm.e2 + p0) : 0.f, c2b = p1 < prm.P ? __ldg(prm.e2 + p1) : 0.f;
+                float acc[R];
+#pragma unroll
+                for (int j = 0; j < R; ++j) acc[j] = 0.f;
+                int prev = 0;
+                for (int kb = 0; kb < nkb; ++kb) {
+                    mbar_wait(XFULL(buf, kb), xpar);
+                    mbar_wait(FULL(stage), phase);
+                    if (!(prm.debug & 4)) {
+                        const uint32_t ph = st_base + (uint32_t)stage * 2 * SUB_BYTES + (uint32_t)wg * 64u * 128u;
+                        const uint32_t pl = ph + SUB_BYTES;
+                        const uint32_t xh = xb + (uint32_t)kb * XSUB, xl = xb + (uint32_t)(nkb + kb) * XSUB;
+                        wg_fence();
+#pragma unroll
+                        for (int k = 0; k < KB / 16; ++k) {
+                            const uint32_t off = (uint32_t)k * 32u;   // 16 fp16 = 32 B inside the 128 B swizzle row
+                            const uint64_t a_h = gmma_desc(ph + off), a_l = gmma_desc(pl + off);
+                            const uint64_t b_h = gmma_desc(xh + off), b_l = gmma_desc(xl + off);
+                            wg_mma_ss<NI>(acc, a_h, b_h);
+                            wg_mma_ss<NI>(acc, a_l, b_h);
+                            wg_mma_ss<NI>(acc, a_h, b_l);
+                        }
+                        wg_commit();
+                    }
+                    if (kb > 0) {                                 // K block kb - 1 has retired: release what it read
+                        wg_wait<1>();
+                        __syncwarp();
+                        if (lane == 0) {
+                            mbar_arrive(EMPTY(prev));
+                            if (last) mbar_arrive(XEMPTY(buf, kb - 1));
+                        }
+                    }
+                    prev = stage;
+                    if (++stage == S) { stage = 0; phase ^= 1u; }
+                }
+                wg_wait<0>();
+                wg_fence_operands(acc);
+                __syncwarp();
+                if (lane == 0) {
+                    mbar_arrive(EMPTY(prev));
+                    if (last) mbar_arrive(XEMPTY(buf, nkb - 1));
+                }
+                if (prm.debug & 8) continue;
+                // v = e0 + e1 acc + e2 |x|^2, the expression and rounding of epilogue_chunk; strict '>' over increasing
+                // columns keeps the first of equal maxima
+                float ma = -INFINITY, mb = -INFINITY;
+                int ia = 0, ib = 0;
+#pragma unroll
+                for (int i = 0; i < NI / 8; ++i) {
+                    const float2 s = *reinterpret_cast<const float2*>(sn + 8 * i + 2 * q);
+#pragma unroll
+                    for (int j = 0; j < 2; ++j) {
+                        const int col = 8 * i + 2 * q + j;
+                        const bool ok = (8 * i + 8 <= HW_MIN) || col < HW;
+                        const float sj = j ? s.y : s.x;
+                        const float va = fmaf(c1a, acc[4 * i + j], fmaf(c2a, sj, c0a));
+                        const float vb = fmaf(c1b, acc[4 * i + 2 + j], fmaf(c2b, sj, c0b));
+                        if (ok && va > ma) { ma = va; ia = col; }
+                        if (ok && vb > mb) { mb = vb; ib = col; }
+                    }
+                }
+#pragma unroll
+                for (int o = 1; o <= 2; o <<= 1) {                // merge the quad: larger value, then smaller column
+                    const float oa = __shfl_xor_sync(0xffffffffu, ma, o), ob = __shfl_xor_sync(0xffffffffu, mb, o);
+                    const int ja = __shfl_xor_sync(0xffffffffu, ia, o), jb = __shfl_xor_sync(0xffffffffu, ib, o);
+                    if (oa > ma || (oa == ma && ja < ia)) { ma = oa; ia = ja; }
+                    if (ob > mb || (ob == mb && jb < ib)) { mb = ob; ib = jb; }
+                }
+                if (q == 0 && (!(prm.debug & 1) || ma + mb == 123.456f)) {
+                    if (p0 < prm.P) best[(size_t)nt * prm.P + p0] = top1_pack(ma, ia);
+                    if (p1 < prm.P) best[(size_t)nt * prm.P + p1] = top1_pack(mb, ib);
+                }
+            }
+        }
     }
 }
 
@@ -647,10 +825,16 @@ int mgp_logprob_tc_launch(const float* xhat, const float* mu, const float* sigma
     // [B,P,HW] through the 3-D map uses image-aligned x tiles (a chunk may not cross an image end)
     const bool tma_bphw = (layout != MGP_OUT_LOGP_NP) && (HW % 4 == 0) && HW >= 32 && HW <= 256 && tma_ok && D <= 128;
     const bool top1 = (layout == MGP_OUT_TOP1_BP);
-    // image-aligned x tiles (box of 32 rows) for the [B,P,HW] TMA stores and for the top-1 epilogue
-    const bool img_tiles = (tma_bphw && !top1) || (top1 && HW >= 32 && HW <= 256 && D <= 128);
+    // top-1 with image tiles (logprob_top1_wide_kernel) unless sigma is known to be anisotropic (x staged with its x^2
+    // half).  Whether sigma is isotropic is otherwise decided on the device (tc_proto_prep_kernel's flag): unless the
+    // caller promised it, the 128-patch-tile kernel is launched behind the wide one and returns at once when it is.
+    const bool iso_known = assume_iso || x_staged == 1;
+    const bool top1_wide = top1 && HW >= 32 && HW <= 256 && (D == 64 || D == 128) && x_staged != 2;
+    const bool top1_tiles = top1 && (!top1_wide || !iso_known);
+    // image-aligned x tiles (box of 32 rows) for the [B,P,HW] TMA stores
+    const bool img_tiles = tma_bphw && !top1;
     const uint32_t xbox = img_tiles ? 32u : 128u;
-    if (top1) MGP_CUDA(cudaMemsetAsync(out, 0, (size_t)B * P * sizeof(unsigned long long), st));
+    if (top1_tiles) MGP_CUDA(cudaMemsetAsync(out, 0, (size_t)B * P * sizeof(unsigned long long), st));
     if (!make_map(&mxh, ah, (uint64_t)N, 2 * D, xbox) || !make_map(&mxl, al, (uint64_t)N, 2 * D, xbox) ||
         !make_map(&mph, bh, (uint64_t)P, 2 * D, 128) || !make_map(&mpl, bl, (uint64_t)P, 2 * D, 128))
         return MGP_ERR_UNSUPPORTED;
@@ -664,6 +848,7 @@ int mgp_logprob_tc_launch(const float* xhat, const float* mu, const float* sigma
     prm.e0 = e0; prm.e1 = e1; prm.e2 = e2; prm.sn = sn; prm.noniso = flag; prm.out = out;
     prm.N = (int)N; prm.HW = HW; prm.P = P; prm.D = D;
     prm.x_no_sq = (x_staged == 1) ? 1 : 0;          // staged without the x^2 half: an anisotropic sigma must fault, not read stale data
+    prm.iso_elsewhere = 0;
     {
         const char* dbg = getenv("MGP_TC_DEBUG");
         prm.debug = dbg ? atoi(dbg) : 0;
@@ -684,19 +869,50 @@ int mgp_logprob_tc_launch(const float* xhat, const float* mu, const float* sigma
     }
     if (team > prm.n_ptiles) team = prm.n_ptiles;
     if (team > sms) team = sms;
-    int n_teams = sms / team;
+    const int n_teams_max = sms / team;
+    prm.team = team;
+    const size_t smem = (size_t)227 * 1024;
+    prm.smem_bytes = (uint32_t)smem;
+
+    if (top1_wide) {
+        // the x map's box is the whole image tile (NI rows, NI = HW rounded up to an instantiated width)
+        const int ni = HW <= 32 ? 32 : HW <= 56 ? 56 : HW <= 64 ? 64 : HW <= 128 ? 128 : HW <= 200 ? 200 : 256;
+        CUtensorMap wxh, wxl;
+        if (!make_map(&wxh, ah, (uint64_t)N, 2 * D, (uint32_t)ni) || !make_map(&wxl, al, (uint64_t)N, 2 * D, (uint32_t)ni))
+            return MGP_ERR_UNSUPPORTED;
+        TcParams pw = prm;
+        pw.iso_elsewhere = iso_known ? 0 : 1;
+        const int grid_w = (n_teams_max < B ? n_teams_max : B) * team;
+#define MGP_TOP1_WIDE(NI, LO)                                                                                      \
+    do {                                                                                                           \
+        MGP_CUDA(cudaFuncSetAttribute(logprob_top1_wide_kernel<NI, LO>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+                                      (int)smem));                                                                 \
+        logprob_top1_wide_kernel<NI, LO><<<grid_w, TC_THREADS, smem, st>>>(wxh, wxl, mph, mpl, pw);               \
+    } while (0)
+        switch (ni) {
+            case 32: MGP_TOP1_WIDE(32, 32); break;
+            case 56: MGP_TOP1_WIDE(56, 33); break;
+            case 64: MGP_TOP1_WIDE(64, 57); break;
+            case 128: MGP_TOP1_WIDE(128, 65); break;
+            case 200: MGP_TOP1_WIDE(200, 129); break;
+            default: MGP_TOP1_WIDE(256, 201); break;
+        }
+#undef MGP_TOP1_WIDE
+        MGP_CHECK_LAUNCH();
+        if (!top1_tiles) return MGP_OK;
+        prm.iso_elsewhere = 1;
+    }
+
+    int n_teams = n_teams_max;
     {
         const int nt_min = (img_tiles && B < prm.n_ntiles) ? B : prm.n_ntiles;
         if (n_teams > nt_min) n_teams = nt_min;
     }
-    prm.team = team;
     const int grid = n_teams * team;
     // shared memory: 1 KiB alignment slack + x tile(s) + prototype stages + 32 KiB staging + 2 KiB misc
     const size_t x_max = (size_t)(assume_iso && D > 128 ? 512 : 1024) * D;   // general: 128 x 2D x 4 B (isotropic: half)
-    if (1024 + x_max + (size_t)2 * 2 * SUB_BYTES + STAGING_BYTES + 2048 > (size_t)227 * 1024)
+    if (1024 + x_max + (size_t)2 * 2 * SUB_BYTES + STAGING_BYTES + 2048 > smem)
         return MGP_ERR_UNSUPPORTED;
-    const size_t smem = (size_t)227 * 1024;
-    prm.smem_bytes = (uint32_t)smem;
 
 #define MGP_TC_LAUNCH(L)                                                                                           \
     do {                                                                                                           \

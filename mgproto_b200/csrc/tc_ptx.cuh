@@ -82,6 +82,61 @@ __device__ __forceinline__ void wg_mma_n16(float (&d)[8], uint64_t a_desc, uint6
         : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TA));
 }
 
+// Image-wide MMAs: D[64 x NI] (+)= A[64 x 16] . B[16 x NI], both K-major in shared memory, accumulator d[NI / 2].
+// wg_mma_ss<NI> exists for the widths MGP_WG_MMA_SS instantiates below.  The asm operand lists are generated:
+// accumulator r is operand %r, so the placeholder "%r" and the constraint "+f"(d[r]) come from the same
+// decimal-digit macros (X(p, u) stands for register pu; p is the leading digits, empty for r < 10).
+template <int NI>
+__device__ __forceinline__ void wg_mma_ss(float (&d)[NI / 2], uint64_t a_desc, uint64_t b_desc);
+
+#define MGP_WG_S0 "%0"
+#define MGP_WG_S(p, u) ", %" #p #u
+#define MGP_WG_F0 "+f"(d[0])
+#define MGP_WG_F(p, u) , "+f"(d[p##u])
+#define MGP_WG_D2(X, p) X(p, 0) X(p, 1)
+#define MGP_WG_D4(X, p) MGP_WG_D2(X, p) X(p, 2) X(p, 3)
+#define MGP_WG_D6(X, p) MGP_WG_D4(X, p) X(p, 4) X(p, 5)
+#define MGP_WG_D8(X, p) MGP_WG_D6(X, p) X(p, 6) X(p, 7)
+#define MGP_WG_D10(X, p) MGP_WG_D8(X, p) X(p, 8) X(p, 9)
+#define MGP_WG_R10(X, X0) X0 X(, 1) X(, 2) X(, 3) X(, 4) X(, 5) X(, 6) X(, 7) X(, 8) X(, 9)
+#define MGP_WG_R50(X, X0) MGP_WG_R10(X, X0) MGP_WG_D10(X, 1) MGP_WG_D10(X, 2) MGP_WG_D10(X, 3) MGP_WG_D10(X, 4)
+#define MGP_WG_R100(X, X0) MGP_WG_R50(X, X0) MGP_WG_D10(X, 5) MGP_WG_D10(X, 6) MGP_WG_D10(X, 7) MGP_WG_D10(X, 8) MGP_WG_D10(X, 9)
+// accumulator registers per width: NI / 2
+#define MGP_WG_ACC16(X, X0) MGP_WG_R10(X, X0) MGP_WG_D6(X, 1)
+#define MGP_WG_ACC28(X, X0) MGP_WG_R10(X, X0) MGP_WG_D10(X, 1) MGP_WG_D8(X, 2)
+#define MGP_WG_ACC32(X, X0) MGP_WG_R10(X, X0) MGP_WG_D10(X, 1) MGP_WG_D10(X, 2) MGP_WG_D2(X, 3)
+#define MGP_WG_ACC64(X, X0) MGP_WG_R50(X, X0) MGP_WG_D10(X, 5) MGP_WG_D4(X, 6)
+#define MGP_WG_ACC100(X, X0) MGP_WG_R100(X, X0)
+#define MGP_WG_ACC128(X, X0) MGP_WG_R100(X, X0) MGP_WG_D10(X, 10) MGP_WG_D10(X, 11) MGP_WG_D8(X, 12)
+// NI, then the operand numbers of the A descriptor, the B descriptor and the scale-d flag (NI / 2, + 1, + 2)
+#define MGP_WG_MMA_SS(NI, OA, OB, OS)                                                                         \
+    template <>                                                                                                \
+    __device__ __forceinline__ void wg_mma_ss<NI>(float (&d)[NI / 2], uint64_t a_desc, uint64_t b_desc) {      \
+        static_assert(OA == NI / 2 && OB == OA + 1 && OS == OA + 2, "operand numbering");                     \
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #OS ", 0;\n\t"                                  \
+                     "wgmma.mma_async.sync.aligned.m64n" #NI "k16.f32.f16.f16 "                              \
+                     "{" MGP_WG_ACC##OA(MGP_WG_S, MGP_WG_S0) "}, %" #OA ", %" #OB ", p, 1, 1, 0, 0;\n\t}"      \
+                     : MGP_WG_ACC##OA(MGP_WG_F, MGP_WG_F0)                                                     \
+                     : "l"(a_desc), "l"(b_desc), "r"(1u));                                                     \
+    }
+MGP_WG_MMA_SS(32, 16, 17, 18)
+MGP_WG_MMA_SS(56, 28, 29, 30)
+MGP_WG_MMA_SS(64, 32, 33, 34)
+MGP_WG_MMA_SS(128, 64, 65, 66)
+MGP_WG_MMA_SS(200, 100, 101, 102)
+MGP_WG_MMA_SS(256, 128, 129, 130)
+#undef MGP_WG_MMA_SS
+
+// Ties the accumulator registers to this point of the program: the compiler may not move their reads or writes across it
+// (after wg_wait, before the epilogue reads the results).
+template <int R>
+__device__ __forceinline__ void wg_fence_operands(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
 // Shared-memory matrix descriptors (sm_90 GMMA): start>>4 at [0,14), LBO>>4 at [16,30), SBO>>4 at [32,46),
 // layout SWIZZLE_128B (1) at [62,64).
 //   K-major, SWIZZLE_128B : 8-row groups of 128 B rows (1024 B) -> SBO = 1024 B; LBO unused (1).  A K step of 16

@@ -1,6 +1,8 @@
 #!/usr/bin/env python
-"""Time the labelled step's max / arg-max log-likelihood kernel (logprob_tc_kernel<top1>, cfg2) with the ablation
-switches of MGP_TC_DEBUG: 1 no global results, 4 no MMAs, 8 no epilogue work, 16 no prototype loads."""
+"""Time the labelled step's max / arg-max log-likelihood kernel (logprob_top1_wide_kernel at cfg2) with the ablation
+switches of MGP_TC_DEBUG: 1 no global results, 4 no MMAs, 8 no epilogue work, 16 no prototype loads.
+The operands are pre-staged without telling the host that sigma is isotropic, so each launch also includes the
+zeroing of the output and the 128-patch-tile kernel, which returns at once (the anisotropic fallback)."""
 import os
 import sys
 
@@ -35,5 +37,5 @@ for dbg in os.environ.get("KA_DEBUGS", "0,2,4,8,16,6,12,10").split(","):
     e1.record()
     torch.cuda.synchronize()
     t = e0.elapsed_time(e1) / 20 * 1e-3
-    print("debug=%-3s %.1f us per launch (memset + kernel, operands pre-staged)  %.0f TFLOP/s equivalent" % (dbg, t * 1e6, flops / t / 1e12))
+    print("debug=%-3s %.1f us per launch (memset + kernels, operands pre-staged)  %.0f TFLOP/s equivalent" % (dbg, t * 1e6, flops / t / 1e12))
 os.environ["MGP_TC_DEBUG"] = "0"
