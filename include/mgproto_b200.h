@@ -61,6 +61,15 @@ extern "C" {
                                   (0xffffffff - hw), ties -> smaller hw.  Tensor-core path only
                                   (MGP_ERR_UNSUPPORTED otherwise); feeds mgp_head_select_top1    */
 
+/* feature formats of the add-on features x [B,D,H,W] (the x_fmt argument of the *_x entry points): element type,
+ * OR-ed with MGP_X_NHWC when x is channels_last, i.e. [B,HW,D] = [N,D] row-major (NCHW, [B,D,HW], otherwise).
+ * torch.autocast makes the add-on convolutions return bf16 / fp16.  Only x and its gradient take these formats:
+ * xhat, inv_norm, the staged operands and the NCHW copy of xhat are fp32 in every format. */
+#define MGP_X_F32 0
+#define MGP_X_BF16 1
+#define MGP_X_F16 2
+#define MGP_X_NHWC 4
+
 int mgp_abi_version(void);
 const char* mgp_error_string(int code);
 /* 1 if the library was built with the sm_90a tensor-core (wgmma) kernels */
@@ -99,6 +108,19 @@ int mgp_normalize_fwd_stage(const float* x_nchw, float* xhat_nd, float* inv_norm
  *   g_x = (g - xhat * <xhat, g>) * inv_norm. */
 int mgp_normalize_bwd(const float* g_xhat_nd, const float* xhat_nd, const float* inv_norm,
                       float* g_x_nchw, int B, int D, int HW, void* stream);
+
+/* Both of the above for features x in any MGP_X_* format (ref: model.py:210-211, :431-432 under torch.autocast,
+ * where F.normalize of bf16 / fp16 add-on features yields fp32).  x_fmt = MGP_X_F32 is exactly mgp_normalize_fwd
+ * (ws == NULL) or mgp_normalize_fwd_stage (ws != NULL; P and stage_aniso are read only then).  16-bit values are
+ * widened on load; every output is fp32 and bit-identical to the MGP_X_F32 pass on the features converted to fp32
+ * NCHW.  An unknown x_fmt returns MGP_ERR_INVALID. */
+int mgp_normalize_fwd_x(const void* x, int x_fmt, float* xhat_nd, float* inv_norm, float* xhat_nchw,
+                        void* ws, size_t ws_bytes, int B, int D, int HW, int P, int stage_aniso,
+                        void* stream);
+/* mgp_normalize_bwd writing g_x in x_fmt's type and layout (the gradient autograd hands back to the add-on
+ * convolutions): the fp32 value of mgp_normalize_bwd, rounded to nearest-even for bf16 / fp16. */
+int mgp_normalize_bwd_x(const float* g_xhat_nd, const float* xhat_nd, const float* inv_norm, void* g_x,
+                        int x_fmt, int B, int D, int HW, void* stream);
 
 /* ---- a2/a3/a16  diagonal-Gaussian log-likelihood -----------------------------------------
  * ref: model.py:256-275 (compute_log_prob, eps = 0), :323-336 (_estimate_log_prob,
@@ -163,6 +185,13 @@ int mgp_head_bwd(const float* grad_logits, const float* logits, const float* val
                  const float* xhat_nd, const float* inv_norm, const float* mu,
                  const float* sigma, void* ws, size_t ws_bytes, float* g_x_nchw, int B, int HW,
                  int C, int K, int D, int T, void* stream);
+/* The same with g_x in the MGP_X_* format x_fmt of the features (ref: model.py:210-222 backward under
+ * torch.autocast): the normalisation backward writes the gradient in x's type and layout (see mgp_normalize_bwd_x). */
+int mgp_head_bwd_x(const float* grad_logits, const float* logits, const float* vals,
+                   const int32_t* idx, const float* weight_cp, const int64_t* gt,
+                   const float* xhat_nd, const float* inv_norm, const float* mu,
+                   const float* sigma, void* ws, size_t ws_bytes, void* g_x, int x_fmt, int B,
+                   int HW, int C, int K, int D, int T, void* stream);
 
 /* ref: model.py:188-206 (global_max_pooling_gmm_topT) as a stand-alone call on PROBABILITIES sims [B,P,HW]:
  * vals [B,P,T] = the T largest over HW, descending; idx [B,P,T] their patch indices; feats [B,P,D,T] (optional, NULL

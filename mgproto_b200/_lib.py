@@ -14,6 +14,7 @@ LIB_PATH = os.path.join(_HERE, "libmgproto_b200.so")
 MGP_MATH_FP32, MGP_MATH_TC, MGP_MATH_AUTO, MGP_MATH_TC_REUSE, MGP_MATH_TC_ISO, MGP_MATH_TC_ISO_REUSE = 0, 1, 2, 3, 4, 5
 MGP_MATH_X_STAGED, MGP_MATH_X_STAGED_ISO = 0x100, 0x200
 MGP_OUT_LOGP_NP, MGP_OUT_LOGP_BPHW, MGP_OUT_NEGP_BPHW, MGP_OUT_TOP1_BP = 0, 1, 2, 3
+MGP_X_F32, MGP_X_BF16, MGP_X_F16, MGP_X_NHWC = 0, 1, 2, 4
 
 _vp, _i, _f, _sz, _d = C.c_void_p, C.c_int, C.c_float, C.c_size_t, C.c_double
 
@@ -28,6 +29,8 @@ SIGNATURES = {
     "mgp_normalize_bwd": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "mgp_logprob_ws_bytes": (_sz, [_i, _i, _i, _i, _i]),
     "mgp_normalize_fwd_stage": (_i, [_vp, _vp, _vp, _vp, _vp, _sz, _i, _i, _i, _i, _i, _vp]),
+    "mgp_normalize_fwd_x": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _sz, _i, _i, _i, _i, _i, _vp]),
+    "mgp_normalize_bwd_x": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "mgp_logprob_ws_is_prototype_only": (_i, [_i, _i, _i, _i]),
     "mgp_logprob_fwd": (_i, [_vp, _vp, _vp, _f, _f, _vp, _i, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
     "mgp_head_select": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
@@ -35,6 +38,7 @@ SIGNATURES = {
     "mgp_head_select_top1": (_i, [_vp] * 9 + [_i] * 6 + [_vp]),
     "mgp_head_bwd_ws_bytes": (_sz, [_i, _i, _i, _i]),
     "mgp_head_bwd": (_i, [_vp] * 11 + [_sz, _vp] + [_i] * 6 + [_vp]),
+    "mgp_head_bwd_x": (_i, [_vp] * 11 + [_sz, _vp] + [_i] * 7 + [_vp]),
     "mgp_mined_gather": (_i, [_vp] * 5 + [_i] * 8 + [_vp]),
     "mgp_bank_enqueue": (_i, [_vp] * 7 + [_i] * 3 + [_vp] * 4 + [_i] * 5 + [_vp]),
     "mgp_bank_enqueue_plan_ints": (_sz, [_i, _i, _i]),

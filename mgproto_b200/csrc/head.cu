@@ -1017,12 +1017,12 @@ extern "C" size_t mgp_head_bwd_ws_bytes(int B, int HW, int P, int D) {
     return ((size_t)2 * P * D + (size_t)B * HW * D + (size_t)P + 64) * sizeof(float);
 }
 
-extern "C" int mgp_head_bwd(const float* grad_logits, const float* logits, const float* vals, const int32_t* idx,
-                            const float* weight_cp, const int64_t* gt, const float* xhat_nd, const float* inv_norm,
-                            const float* mu, const float* sigma, void* ws, size_t ws_bytes, float* g_x_nchw, int B,
-                            int HW, int C, int K, int D, int T, void* stream) {
+extern "C" int mgp_head_bwd_x(const float* grad_logits, const float* logits, const float* vals, const int32_t* idx,
+                              const float* weight_cp, const int64_t* gt, const float* xhat_nd, const float* inv_norm,
+                              const float* mu, const float* sigma, void* ws, size_t ws_bytes, void* g_x, int x_fmt,
+                              int B, int HW, int C, int K, int D, int T, void* stream) {
     if (!grad_logits || !logits || !vals || !idx || !weight_cp || !xhat_nd || !inv_norm || !mu || !sigma || !ws ||
-        !g_x_nchw)
+        !g_x || !mgp_x_fmt_valid(x_fmt))
         return MGP_ERR_INVALID;
     if (B <= 0 || HW <= 0 || C <= 0 || K <= 0 || D <= 0 || T <= 0) return MGP_ERR_INVALID;
     if (HW > 1024 || (size_t)C * K >= (1u << 22)) return MGP_ERR_UNSUPPORTED;
@@ -1054,7 +1054,15 @@ extern "C" int mgp_head_bwd(const float* grad_logits, const float* logits, const
         head_bwd_kernel<2><<<grid, 256, smem, st>>>(grad_logits, logits, vals, idx, weight_cp, gt, xhat_nd, w, wm, wsc, noniso,
                                                     g_xhat, HW, C, K, D, T);
     MGP_CHECK_LAUNCH();
-    return mgp_normalize_bwd(g_xhat, xhat_nd, inv_norm, g_x_nchw, B, D, HW, stream);
+    return mgp_normalize_bwd_x(g_xhat, xhat_nd, inv_norm, g_x, x_fmt, B, D, HW, stream);
+}
+
+extern "C" int mgp_head_bwd(const float* grad_logits, const float* logits, const float* vals, const int32_t* idx,
+                            const float* weight_cp, const int64_t* gt, const float* xhat_nd, const float* inv_norm,
+                            const float* mu, const float* sigma, void* ws, size_t ws_bytes, float* g_x_nchw, int B,
+                            int HW, int C, int K, int D, int T, void* stream) {
+    return mgp_head_bwd_x(grad_logits, logits, vals, idx, weight_cp, gt, xhat_nd, inv_norm, mu, sigma, ws, ws_bytes,
+                          g_x_nchw, MGP_X_F32, B, HW, C, K, D, T, stream);
 }
 
 extern "C" int mgp_mine_ce(const float* out, const int64_t* gt, float* loss_b, float* grad, int B, int C, int T,

@@ -21,6 +21,8 @@
     } while (0)
 
 static inline bool mgp_aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+// MGP_X_F32 / _BF16 / _F16, optionally | MGP_X_NHWC
+static inline bool mgp_x_fmt_valid(int f) { return f >= 0 && (f & ~MGP_X_NHWC) <= MGP_X_F16; }
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

@@ -215,7 +215,7 @@ class MGProto(nn.Module):
     def push_forward_features(self, x_add):
         C, K, D = self.prototype_means.shape
         B, _, H, W = x_add.shape
-        xhat, _, nchw = ops.normalize_fwd(x_add.contiguous(), want_nchw=True)
+        xhat, _, nchw = ops.normalize_fwd(x_add, want_nchw=True)
         dist = ops.logprob(xhat, self.prototype_means.detach().reshape(C * K, D),
                            self.prototype_covs.detach().reshape(C * K, D), MGP_OUT_NEGP_BPHW, B=B, HW=H * W,
                            math=self.math_mode)
@@ -232,10 +232,10 @@ class MGProto(nn.Module):
         # the max / arg-max epilogue of the tensor-core kernel already is the per-prototype search: no [B,P,HW] map at all
         stage = ops._stage_for_top1(B, H * W, C * K, D, sg, self.math_mode)
         if stage is not None:
-            xhat, _, _, ws = ops.normalize_fwd(x_add.contiguous(), stage=stage)
+            xhat, _, _, ws = ops.normalize_fwd(x_add, stage=stage)
             best = ops.logprob_top1(xhat, mu, sg, B, H * W, self.math_mode, ws=ws, staged=stage)
         else:
-            xhat, _, _ = ops.normalize_fwd(x_add.contiguous())
+            xhat, _, _ = ops.normalize_fwd(x_add)
             best = ops.logprob_top1(xhat, mu, sg, B, H * W, self.math_mode)
         if best is not None:
             arg, val = ops.push_argmin_top1(best, labels.contiguous(), C, K)

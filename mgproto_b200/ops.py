@@ -15,7 +15,8 @@ from . import _lib
 from ._lib import (MGP_MATH_AUTO, MGP_MATH_FP32, MGP_MATH_TC, MGP_MATH_TC_ISO, MGP_MATH_TC_ISO_REUSE, MGP_MATH_TC_REUSE,
                    MGP_MATH_X_STAGED, MGP_MATH_X_STAGED_ISO,
                    MGP_OUT_LOGP_BPHW,
-                   MGP_OUT_LOGP_NP, MGP_OUT_NEGP_BPHW, MGP_OUT_TOP1_BP, check)
+                   MGP_OUT_LOGP_NP, MGP_OUT_NEGP_BPHW, MGP_OUT_TOP1_BP, MGP_X_BF16, MGP_X_F16, MGP_X_F32, MGP_X_NHWC,
+                   check)
 
 __all__ = ["normalize_fwd", "logprob", "logprob_top1", "head_select", "head_select_top1", "head_level0", "head_forward", "HeadFunction", "mined_gather", "bank_enqueue",
            "bank_linearize", "bank_shadow_sync", "em_plan", "em_stats", "em_update", "update_gmm", "em_estep", "em_mstep_closed", "em_mstep_div", "topt_pool", "ood_score", "push_argmin", "push_argmin_top1", "mine_cross_entropy",
@@ -137,30 +138,45 @@ def _math(math) -> int:
 
 
 # ----------------------------------------------------------------------------------- a1
+_FEATURE_DTYPES = {torch.float32: MGP_X_F32, torch.bfloat16: MGP_X_BF16, torch.float16: MGP_X_F16}
+
+
+def _feature_format(x: torch.Tensor):
+    """Add-on features [B,D,H,W] -> (x, x_fmt): the MGP_X_* code of x's dtype, | MGP_X_NHWC when x is channels_last
+    (torch.autocast returns the add-on convolutions' output in bf16 / fp16, often channels_last).  Any other stride
+    pattern is made contiguous NCHW; any other dtype raises."""
+    code = _FEATURE_DTYPES.get(x.dtype)
+    if code is None:
+        raise RuntimeError("mgproto_b200: x must be torch.float32, torch.bfloat16 or torch.float16, got %s" % x.dtype)
+    if x.dim() == 4 and not x.is_contiguous() and x.is_contiguous(memory_format=torch.channels_last):
+        return x, code | MGP_X_NHWC
+    return x.contiguous(), code
+
+
 @_on_device
 def normalize_fwd(x_bdhw: torch.Tensor, want_nchw: bool = False, stage=None):
-    """ref model.py:210-211.  -> (xhat [N,D], inv_norm [N], xhat_nchw [B,D,H,W] | None).
+    """ref model.py:210-211.  x [B,D,H,W] in fp32 / bf16 / fp16, NCHW or channels_last (_feature_format) ->
+    (xhat [N,D], inv_norm [N], xhat_nchw [B,D,H,W] | None), all fp32 and contiguous.
     stage = (P, aniso): also write the patch-side operands of the tensor-core log-likelihood kernels in the same pass
-    (mgp_normalize_fwd_stage) -> a 4th return value: the workspace to hand to logprob_top1(..., staged=...)."""
-    x = _req(x_bdhw, torch.float32, "x")
+    -> a 4th return value: the workspace to hand to logprob_top1(..., staged=...)."""
+    if not isinstance(x_bdhw, torch.Tensor) or not x_bdhw.is_cuda:
+        raise RuntimeError("mgproto_b200: x must be a CUDA tensor (there is no CPU path)")
+    x, fmt = _feature_format(x_bdhw)
     B, D, H, W = x.shape
     HW = H * W
     xhat = torch.empty((B * HW, D), device=x.device, dtype=torch.float32)
     inv = torch.empty((B * HW,), device=x.device, dtype=torch.float32)
-    nchw = torch.empty_like(x) if want_nchw else None
+    nchw = torch.empty((B, D, H, W), device=x.device, dtype=torch.float32) if want_nchw else None
     lib = _lib.load()
+    ws, nbytes, P, aniso = None, 0, 0, False
     if stage is not None:
         P, aniso = stage
         nbytes = lib.mgp_logprob_ws_bytes(B, HW, int(P), D, MGP_MATH_TC)
         ws = torch.empty((max(16, nbytes),), device=x.device, dtype=torch.uint8)
-        check(lib.mgp_normalize_fwd_stage(x.data_ptr(), xhat.data_ptr(), inv.data_ptr(), _p(nchw), ws.data_ptr(), nbytes,
-                                          B, D, HW, int(P), 1 if aniso else 0, _stream()), "mgp_normalize_fwd_stage")
-        _count(1)
-        return xhat, inv, nchw, ws
-    check(lib.mgp_normalize_fwd(x.data_ptr(), xhat.data_ptr(), inv.data_ptr(), _p(nchw), B, D, HW, _stream()),
-          "mgp_normalize_fwd")
+    check(lib.mgp_normalize_fwd_x(x.data_ptr(), fmt, xhat.data_ptr(), inv.data_ptr(), _p(nchw), _p(ws), nbytes,
+                                  B, D, HW, int(P), 1 if aniso else 0, _stream()), "mgp_normalize_fwd_x")
     _count(1)
-    return xhat, inv, nchw
+    return (xhat, inv, nchw, ws) if stage is not None else (xhat, inv, nchw)
 
 
 def _stage_for_top1(B, HW, P, D, sg, math):
@@ -329,6 +345,8 @@ class HeadFunction(torch.autograd.Function):
     model.py:264-265; last_layer.weight has requires_grad=False) by re-differentiating the T
     selected patches per (image, prototype) instead of saving the N*P*D autograd tape.
     Also returns (non-differentiable) xhat [N,D] and idx [B,P,T] for the bank enqueue.
+    The features may be fp32 / bf16 / fp16, NCHW or channels_last (_feature_format): they are read
+    as they are, and their gradient comes back in the same dtype and memory format.
     """
 
     @staticmethod
@@ -336,7 +354,7 @@ class HeadFunction(torch.autograd.Function):
         C, K, D = mu_ckd.shape
         B, _, H, W = x_add.shape
         HW = H * W
-        x_add = x_add.contiguous()
+        x_add, x_fmt = _feature_format(x_add)
         mu = mu_ckd.detach().reshape(C * K, D).contiguous()
         sg = sigma_ckd.detach().reshape(C * K, D).contiguous()
         wt = weight_cp.detach().contiguous()
@@ -359,6 +377,7 @@ class HeadFunction(torch.autograd.Function):
         ctx.save_for_backward(logits, vals, idx, wt, gt if gt is not None else torch.empty(0), xhat, inv, mu, sg)
         ctx.has_gt = gt is not None
         ctx.dims = (B, HW, C, K, D, T, H, W)
+        ctx.x_fmt = x_fmt
         ctx.mark_non_differentiable(xhat, idx)
         ctx.set_materialize_grads(False)      # no zero-filled "gradients" for xhat [N,D] / idx [B,P,T] (67 MB of fills)
         return logits, xhat, idx
@@ -369,22 +388,28 @@ class HeadFunction(torch.autograd.Function):
             return (None,) * 7
         logits, vals, idx, wt, gt, xhat, inv, mu, sg = ctx.saved_tensors
         B, HW, C, K, D, T, H, W = ctx.dims
-        gx = head_backward(g_logits, logits, vals, idx, wt, gt if ctx.has_gt else None, xhat, inv, mu, sg, ctx.dims)
+        gx = head_backward(g_logits, logits, vals, idx, wt, gt if ctx.has_gt else None, xhat, inv, mu, sg, ctx.dims,
+                           ctx.x_fmt)
         return gx, None, None, None, None, None, None
 
 
+_X_DTYPES = {v: k for k, v in _FEATURE_DTYPES.items()}
+
+
 @_on_device
-def head_backward(g_logits, logits, vals, idx, wt, gt, xhat, inv, mu, sg, dims):
-    """d logits / d features through the selected patches only (mgp_head_bwd): -> grad of the add-on features [B,D,H,W]."""
+def head_backward(g_logits, logits, vals, idx, wt, gt, xhat, inv, mu, sg, dims, x_fmt=MGP_X_F32):
+    """d logits / d features through the selected patches only (mgp_head_bwd_x): -> grad of the add-on features
+    [B,D,H,W] in the dtype and memory format that x_fmt (_feature_format) names."""
     B, HW, C, K, D, T, H, W = dims
     g = _req(g_logits.contiguous(), torch.float32, "grad_logits")
     lib = _lib.load()
     nbytes = lib.mgp_head_bwd_ws_bytes(B, HW, C * K, D)
     ws = torch.empty((nbytes,), device=g.device, dtype=torch.uint8)
-    gx = torch.empty((B, D, H, W), device=g.device, dtype=torch.float32)
-    check(lib.mgp_head_bwd(g.data_ptr(), logits.data_ptr(), vals.data_ptr(), idx.data_ptr(), wt.data_ptr(), _p(gt),
-                           xhat.data_ptr(), inv.data_ptr(), mu.data_ptr(), sg.data_ptr(), ws.data_ptr(), nbytes,
-                           gx.data_ptr(), B, HW, C, K, D, T, _stream()), "mgp_head_bwd")
+    mf = torch.channels_last if x_fmt & MGP_X_NHWC else torch.contiguous_format
+    gx = torch.empty((B, D, H, W), device=g.device, dtype=_X_DTYPES[x_fmt & ~MGP_X_NHWC], memory_format=mf)
+    check(lib.mgp_head_bwd_x(g.data_ptr(), logits.data_ptr(), vals.data_ptr(), idx.data_ptr(), wt.data_ptr(), _p(gt),
+                             xhat.data_ptr(), inv.data_ptr(), mu.data_ptr(), sg.data_ptr(), ws.data_ptr(), nbytes,
+                             gx.data_ptr(), int(x_fmt), B, HW, C, K, D, T, _stream()), "mgp_head_bwd_x")
     _count(3)
     return gx
 
@@ -403,10 +428,10 @@ def head_level0(x_add, mu_ckd, sigma_ckd, weight_cp, math="auto"):
         fits = HW <= 1024 and (2 * C * K + 2 * K + K * (HW + 1) + 2 * K * D + 2 * K + 4) * 4 <= 200 * 1024
         stage = _stage_for_top1(B, HW, C * K, D, sg, math) if fits else None
         if stage is not None:
-            xhat, _, _, ws1 = normalize_fwd(x_add.detach().contiguous(), stage=stage)
+            xhat, _, _, ws1 = normalize_fwd(x_add.detach(), stage=stage)
             best = logprob_top1(xhat, mu, sg, B, HW, math, ws=ws1, staged=stage)
         else:
-            xhat, _, _ = normalize_fwd(x_add.detach().contiguous())
+            xhat, _, _ = normalize_fwd(x_add.detach())
             best = logprob_top1(xhat, mu, sg, B, HW, math) if fits else None
         if best is None:
             lp = logprob(xhat, mu, sg, MGP_OUT_LOGP_BPHW, B=B, HW=HW, math=math)
