@@ -1211,7 +1211,8 @@ em_update_kernel(const float* __restrict__ stats, int n_split, size_t stat_strid
     }
     __syncthreads();
     const float n_rows = (float)n_rows_total;
-    const float div_scale = -4.0f * lamda / ((float)K * (float)(K - 1));
+    // K = 1 has no prototype pairs: no diversity term (the reference's mean over the empty pair set is 0/0, NaN)
+    const float div_scale = (K > 1) ? -4.0f * lamda / ((float)K * (float)(K - 1)) : 0.f;
     const int step = step0 + num_em_loop * ord + em_loop + 1;
     const double b1p = pow(adam.beta1, (double)step), b2p = pow(adam.beta2, (double)step);
     // all global operands of up to 8 owned elements are fetched before any is used (the kernel is a chain of

@@ -8,7 +8,7 @@ import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
 
-SHAPES = [(14, 14), (7, 7), (16, 16), (10, 10), (3, 11), (4, 8)]   # HW = 196, 49, 256, 100, 33, 32
+SHAPES = [(14, 14), (7, 7), (16, 16), (10, 10), (3, 11), (4, 8), (8, 8), (7, 9)]   # HW = 196, 49, 256, 100, 33, 32, 64, 63
 B, P = 37, 2000        # 37 images do not divide into the teams of the schedule; the last prototype tile is partial
 
 
@@ -36,8 +36,9 @@ def _unpack(best):
 
 @pytest.mark.parametrize("D", [128, 64])
 @pytest.mark.parametrize("H,W", SHAPES)
-def test_top1_image_tiles_vs_materialised(H, W, D):
+def test_top1_image_tiles_vs_materialised(request, H, W, D):
     from mgproto_b200 import _lib, ops
+    from test_gpu_shape_edges import assert_reached, trace
     HW = H * W
     g = torch.Generator().manual_seed(1000 * HW + D)
     x = torch.randn(B, D, H, W, generator=g).to(_dev())
@@ -45,8 +46,11 @@ def test_top1_image_tiles_vs_materialised(H, W, D):
     sg = torch.full((P, D), 1 / np.sqrt(2 * np.pi), device=_dev())
     xhat, _, _ = ops.normalize_fwd(x)
 
-    # unstaged route: operands prepared by the kernel's own pre-passes
-    best = ops.logprob_top1(xhat, mu, sg, B, HW, "tc")
+    # unstaged route: operands prepared by the kernel's own pre-passes (the trace proves the launch of the image-tile
+    # instantiation for this width; the 128-patch-tile kernel is launched behind it and returns at once)
+    with trace() as tr:
+        best = ops.logprob_top1(xhat, mu, sg, B, HW, "tc")
+    assert_reached(request, tr)
     assert best is not None
     lp = ops.logprob(xhat, mu, sg, 1, B=B, HW=HW, math="tc")
     np.testing.assert_array_equal(best.cpu().numpy(), _pack_first_max(lp))
