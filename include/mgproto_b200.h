@@ -78,9 +78,6 @@ int mgp_has_tensor_core_path(void);
  * key "tc_z": 1 (default; 0 if MGP_TC_NO_Z is set) = the [N,P] log-likelihood with isotropic sigma and D <= 128 takes the
  * register-resident kernel (csrc/logprob_tcz.cu), 0 = always csrc/logprob_tc.cu;
  * key "em_tc": 1 (default; 0 if MGP_EM_NO_TC is set) = mgp_update_gmm may take the tensor-core kernel;
- * key "em_pipe": 1 (default; 0 if MGP_EM_NO_PIPE is set) = at D = 128 that kernel is the software-pipelined variant
- * (three row-tile buffers) while the active classes fit one CTA per SM, and the one-warpgroup variant (two CTAs per SM)
- * beyond; 0 = always the one-warpgroup variant (D = 256 always runs its serial two-warpgroup kernel);
  * key "em_fused": 1 (default; 0 if MGP_EM_UNFUSED is set in the environment) = mgp_update_gmm runs the single
  * cluster launch where the shape allows, 0 = always the multi-launch path (identical arithmetic, used by the
  * parity tests to cross-check the two).  Returns the previous value, or MGP_ERR_INVALID for an unknown key. */

@@ -49,18 +49,8 @@ int mgp_opt_em_tc() {
     if (g_mgp_em_tc < 0) g_mgp_em_tc = getenv("MGP_EM_NO_TC") ? 0 : 1;
     return g_mgp_em_tc;
 }
-int g_mgp_em_pipe = -1;
-int mgp_opt_em_pipe() {
-    if (g_mgp_em_pipe < 0) g_mgp_em_pipe = getenv("MGP_EM_NO_PIPE") ? 0 : 1;
-    return g_mgp_em_pipe;
-}
 extern "C" int mgp_set_option(const char* key, int value) {
     if (!key) return MGP_ERR_INVALID;
-    if (strcmp(key, "em_pipe") == 0) {
-        const int prev = mgp_opt_em_pipe();
-        g_mgp_em_pipe = value ? 1 : 0;
-        return prev;
-    }
     if (strcmp(key, "tc_z") == 0) {
         const int prev = mgp_opt_tc_z();
         g_mgp_tc_z = value ? 1 : 0;

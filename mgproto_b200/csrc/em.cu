@@ -25,7 +25,6 @@ namespace cg = cooperative_groups;
 
 int mgp_opt_em_fused();   // abi.cu
 int mgp_opt_em_tc();      // abi.cu
-int mgp_opt_em_pipe();    // abi.cu
 // em_tc.cu
 bool mgp_em_tc_supported(int K, int D, int cap);
 int mgp_em_tc_launch(const void* shadow_h, const void* shadow_l, const float* shadow_xx, const float* bias_corr, const int32_t* order,
@@ -1465,7 +1464,7 @@ static bool em_tc_applies(int K, int D, int cap, int have_shadow_iso) {
 }
 
 extern "C" int mgp_update_gmm_launches(int K, int D, int cap, int num_em_loop, int have_shadow_iso) {
-    if (em_tc_applies(K, D, cap, have_shadow_iso)) return (D == 128 && mgp_opt_em_pipe()) ? 3 : 2;   // plan + kernel(s)
+    if (em_tc_applies(K, D, cap, have_shadow_iso)) return 2;         // plan + kernel
     return em_fused_applies(K, D, cap) ? 2 : 3 + 2 * num_em_loop;
 }
 

@@ -20,18 +20,17 @@
 // The E-step of a row tile (per m64 half: m64n32 with the X hi rows against [means hi ; means lo], m64n16 with the
 // X lo rows against means hi) is followed by its soft-max straight from the accumulator fragments (the 16 components
 // of a row sit in 4 lanes) and the statistics GEMM of the tile (D / 64 m64 blocks), which keeps S1 in registers across
-// the tiles of a loop; at the end of a loop S1 goes to the owners through shared memory.  Three variants of the same
-// kernel (template flag PIPE, and D):
-//   * serial, D = 256: two warpgroups, 128-row tiles, one tile buffer.  Warpgroup 0 (warps 0-3) runs the E-step and
-//     soft-max, then warpgroup 1 (warps 4-7) the statistics of the tile;
-//   * serial, D = 128 (more classes active than there are SMs): ONE warpgroup of 128 threads runs E-step, soft-max and
-//     statistics of a tile in turn (the two warpgroups above never overlap anyway), so that two CTAs share an SM and
-//     up to 2 x #SMs classes run in one wave.  64-row tiles -- tile t is the half t % 2 of a 128-row tile, so the MMAs
-//     into S1 come in the same order -- stream through a two-slot ring: the TMA load of tile t+1 runs under tile t;
-//   * pipelined (D = 128, one CTA per SM, classes in the planner's order): two warpgroups as in the first variant,
-//     three tile buffers and two R buffers; the TMA load of tile t+1 and the statistics of tile t-1 run under the
-//     E-step and soft-max of tile t.
-// At D = 128 both are enqueued and the planner's count of active classes decides on the device which one does the work.
+// the tiles of a loop; at the end of a loop S1 goes to the owners through shared memory.  Two variants of the same
+// kernel, by D:
+//   * D = 128: ONE warpgroup of 128 threads runs E-step, soft-max and statistics of a tile in turn, so that two CTAs
+//     share an SM and up to 2 x #SMs classes run in one wave.  64-row tiles -- tile t is the half t % 2 of a 128-row
+//     tile, so the MMAs into S1 come in the same order -- stream through a two-slot ring: the TMA load of tile t+1
+//     runs under tile t;
+//   * D = 256: two warpgroups, 128-row tiles, one tile buffer.  Warpgroup 0 (warps 0-3) runs the E-step and soft-max,
+//     then warpgroup 1 (warps 4-7) the statistics of the tile.
+// At D = 128 block b runs class clist[b], the planner's order with the active classes first: they take the lowest
+// block indices, so while they fit one CTA per SM none shares its SM with another active class.  At D = 256 (one CTA
+// per SM in any case) block b runs class b.
 // HBM/L2 traffic: num_em_loop x (4 D + 4) bytes per bank row -- the algorithmic bytes of SURVEY 8(d) K-D.
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -48,11 +47,11 @@ constexpr float SX = 256.0f;      // shadow rows hold 256 x (fp16 hi + lo)
 constexpr float SR = 1024.0f;     // responsibilities are stored as 1024 r
 constexpr int S1_STRIDE = 17;     // S1 hand-over [D][17] fp32 (padded against bank conflicts)
 
-// the serial kernel at D = 128 is the one-warpgroup variant (two CTAs per SM, 64-row tiles); the others have two
+// the kernel at D = 128 is the one-warpgroup variant (two CTAs per SM, 64-row tiles); at D = 256 it has two
 // warpgroups and 128-row tiles (bank rows per tile = M of the E-step, K extent of the statistics GEMM)
-__host__ __device__ constexpr bool em_one_wg(int D, bool pipe) { return !pipe && D == 128; }
-__host__ __device__ constexpr int em_threads(int D, bool pipe) { return em_one_wg(D, pipe) ? 128 : 256; }
-__host__ __device__ constexpr int em_rows(int D, bool pipe) { return em_one_wg(D, pipe) ? 64 : 128; }
+__host__ __device__ constexpr bool em_one_wg(int D) { return D == 128; }
+__host__ __device__ constexpr int em_threads(int D) { return em_one_wg(D) ? 128 : 256; }
+__host__ __device__ constexpr int em_rows(int D) { return em_one_wg(D) ? 64 : 128; }
 
 struct EmTcParams {
     const float* xx;              // [C*cap] |x|^2 of the bank rows (shadow)
@@ -60,7 +59,6 @@ struct EmTcParams {
     const int32_t* order;
     const int32_t* sched;
     const int32_t* clist;         // planner: classes in launch order, active first (stats scratch at 5 L C + 4)
-    int pipe_max;                 // the pipelined kernel runs iff n_active <= pipe_max (0: never)
     float* mu;
     const float* sigma;
     float* weight;
@@ -76,7 +74,7 @@ struct EmTcParams {
 // 5 statistics MMAs done, 6 loop tail entered, 7 loop tail done
 #define MGP_PROF(ctr, ph)                                                                          \
     do {                                                                                           \
-        if (prm.prof && blockIdx.x == prm.prof_class && (ctr) < 64) prm.prof[(ctr) * 8 + (ph)] = clock64();  \
+        if (prm.prof && c == prm.prof_class && (ctr) < 64) prm.prof[(ctr) * 8 + (ph)] = clock64();  \
     } while (0)
 
 // Sum V = 32 R values per lane across the warp with V - R shuffles (a butterfly that halves the live set each round)
@@ -95,12 +93,12 @@ __device__ __forceinline__ void warp_multi_reduce(float (&a)[V], int lane) {
     }
 }
 
-template <int D, int KT, bool PIPE>
-__global__ void __launch_bounds__(em_threads(D, PIPE), em_one_wg(D, PIPE) ? 2 : 1)
+template <int D, int KT>
+__global__ void __launch_bounds__(em_threads(D), em_one_wg(D) ? 2 : 1)
 em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_l, const EmTcParams prm) {
-    constexpr bool WG1 = em_one_wg(D, PIPE);       // one warpgroup runs everything (serial, D = 128)
-    constexpr int NT = em_threads(D, PIPE), NW = NT / 32;
-    constexpr int TR = em_rows(D, PIPE);           // bank rows per tile
+    constexpr bool WG1 = em_one_wg(D);             // one warpgroup runs everything (D = 128)
+    constexpr int NT = em_threads(D), NW = NT / 32;
+    constexpr int TR = em_rows(D);                 // bank rows per tile
     constexpr int NCH = D / 64;                    // 64-element (128 B) chunks along d
     constexpr uint32_t CH_BYTES = TR * 128;        // one [TR rows x 64] fp16 block
     constexpr uint32_t X_BYTES = NCH * CH_BYTES;   // hi (lo follows)
@@ -115,16 +113,15 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
     const uint32_t base = (raw + 1023u) & ~1023u;
     uint8_t* bp = smem_raw + (base - raw);
     // carve-up (bytes from `base`)
-    constexpr int NXBUF = PIPE ? 3 : (WG1 ? 2 : 1), NRBUF = PIPE ? 2 : 1;
+    constexpr int NXBUF = WG1 ? 2 : 1;
     const uint32_t o_xh = 0, o_xl = X_BYTES;                               // buffer b: + b * 2 * X_BYTES
     // means operand A and responsibilities R: per 64-wide K chunk one [32 rows x 128 B] block, rows 0-15 = hi,
     // rows 16-31 = lo, so ONE N = 32 MMA multiplies the row tile's hi half with both and an N = 16 MMA adds lo x hi
     const uint32_t o_a = NXBUF * 2 * X_BYTES;                             // [NCH][32][128 B]
-    const uint32_t o_r = o_a + NCH * 4096;                                // NRBUF x [TR / 64 (64-row chunks)][32][128 B]
-    // S1 hand-over [D][S1_STRIDE]: its own region (!PIPE) or, PIPE, the tile buffer that is idle at the end of a loop
-    const uint32_t o_s1 = o_r + NRBUF * R_BYTES;
-    const uint32_t o_misc = o_s1 + (PIPE ? 0u : (uint32_t)((D * S1_STRIDE * 4 + 15) & ~15));
-    // serial: tma, (unused), stats | one warpgroup: xfull[2] | PIPE: xfull[3] xfree[3] (unused)[2] rfull[2]
+    const uint32_t o_r = o_a + NCH * 4096;                                // [TR / 64 (64-row chunks)][32][128 B]
+    const uint32_t o_s1 = o_r + R_BYTES;                                  // S1 hand-over [D][S1_STRIDE]
+    const uint32_t o_misc = o_s1 + (uint32_t)((D * S1_STRIDE * 4 + 15) & ~15);
+    // two warpgroups: tma, (unused), stats | one warpgroup: xfull[2]
     uint64_t* bars = reinterpret_cast<uint64_t*>(bp + o_misc);
     float* s_e = reinterpret_cast<float*>(bars + 12);                     // [KT][KT]
     float* s_red = s_e + KT * KT;                                         // [8] + [8][16]
@@ -142,15 +139,10 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
     const uint32_t bar_tma = smem_u32(bars), bar_s = bar_tma + 16;
 
     const int n_active = prm.sched[0], step0 = prm.sched[1];
-    // PIPE: one CTA per SM, so the planner's class list (active classes first, in order) decides who starts first
-    // Launch regimes (both kernels are enqueued when D = 128; the planner's count decides on the device):
-    //   n_active <= pipe_max (one CTA per SM covers every active class) -> the pipelined kernel, else the serial one.
-    if (PIPE ? (n_active > prm.pipe_max) : (n_active <= prm.pipe_max)) return;
-    // PIPE: CTA b < n_active runs active class clist[b]; its idle warps also take the inactive classes clist[n_active + b
-    // (+ n_active)], so that those do not queue behind the 225 KB CTAs; inactive classes beyond 2 n_active get own CTAs
-    constexpr int ABSORB = 2;
-    if (PIPE && (int)blockIdx.x >= n_active && (int)blockIdx.x - n_active < ABSORB * n_active) return;
-    const int c = PIPE ? prm.clist[blockIdx.x] : (int)blockIdx.x;
+    // two CTAs per SM (D = 128): the active classes first (the planner's order), so that no two share an SM while
+    // they fit one per SM.  D = 256 runs one CTA per SM and keeps class order: the planner's order measured up to 3 %
+    // slower there at some active counts (DESIGN 8.3)
+    const int c = WG1 ? prm.clist[blockIdx.x] : (int)blockIdx.x;
     const int ord = prm.order[c];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int K = prm.K, cap = prm.cap, L = prm.num_em_loop, P = prm.C * K, KD = K * D;
@@ -257,24 +249,6 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
 #pragma unroll
         for (int k = 0; k < KT; ++k) { m_[k] *= mdec; v_[k] *= vdec; }
     };
-    // an inactive class only takes everybody's zero-gradient steps: warps [w0, w0 + nw) of this CTA, straight from / to
-    // global memory (PIPE: done by the warps that idle during an active class's first tile loop)
-    auto replay_inactive = [&](int ci, int w0, int nw) {
-        const int count = L * n_active;
-        if (count <= 0) return;
-        const int ns = replay_explicit_steps(count, step0, (float)adam.beta1);
-        const bool tail = count > ns;
-        float T1, T2, T3, dmin;
-        replay_sums(step0, count, ns, tail, T1, T2, T3, dmin);            // (every warp for itself: no block barrier here)
-        const float mdec = __ldg(t_b1 + count), vdec = __ldg(t_b2 + count);
-        for (int o = (warp - w0) * 32 + lane; o < KD; o += nw * 32) {
-            const size_t g = (size_t)ci * KD + o;
-            const float p = prm.mu[g], m = prm.exp_avg[g], v = prm.exp_avg_sq[g];
-            prm.mu[g] = replay_elem(p, m, v, step0, count, ns, tail, T1, T2, T3, dmin);
-            prm.exp_avg[g] = m * mdec;
-            prm.exp_avg_sq[g] = v * vdec;
-        }
-    };
     auto write_back = [&]() {
         if (!own) return;
 #pragma unroll
@@ -299,10 +273,7 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
     if (tid == 0) MGP_PROF(63, 1);
     // ---- set-up: barriers, sigma-derived constants, zeroed operand tiles
     if (tid == 0) {
-        if (PIPE) {                                  // xfree / rfull: one arrive per warp of the consuming warpgroup
-            for (int i = 0; i < 3; ++i) { mbar_init(bar_tma + 8u * i, 1); mbar_init(bar_tma + 8u * (3 + i), 4); }
-            for (int i = 0; i < 2; ++i) mbar_init(bar_tma + 8u * (8 + i), 4);
-        } else if (WG1) {
+        if (WG1) {
             for (int i = 0; i < 2; ++i) mbar_init(bar_tma + 8u * i, 1);
         } else {
             mbar_init(bar_tma, 1);
@@ -312,7 +283,7 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
     }
     bool same = true;
     for (int i = tid; i < KD; i += NT) same = same && (sg_c[i] == sg_c[(i / D) * D]);
-    for (uint32_t i = tid * 16u; i < NCH * 4096u + NRBUF * R_BYTES; i += NT * 16u)     // A and R blocks: rows >= K stay zero
+    for (uint32_t i = tid * 16u; i < NCH * 4096u + R_BYTES; i += NT * 16u)     // A and R blocks: rows >= K stay zero
         *reinterpret_cast<uint4*>(bp + o_a + i) = make_uint4(0u, 0u, 0u, 0u);
     for (int i = tid; i < KT * KT; i += NT) s_e[i] = 0.f;
     if (tid < 16) {
@@ -352,9 +323,9 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
     // E-step of one tile + soft-max + R (warps 0-3).  E-step: A = X (K-major), B = [means hi ; means lo] (K-major):
     // N = 32 with X hi, N = 16 (means hi only) with X lo; rows h * 64 + 16 warp + g8 + 8 rr of the tile (NH m64
     // halves), components k = 8 i + 2 t4 + j (columns k: hi.hi, 16 + k: hi.lo; the N = 16 accumulator: lo.hi).
-    // before_write() runs between the soft-max and the R stores (PIPE: wait until the R buffer is free)
     constexpr int NH = TR / 64;
-    auto estep_tile = [&](uint32_t xb, uint8_t* rbp, int t, float inv_a, float (&s0v)[4], auto&& before_write) {
+    auto estep_tile = [&](uint32_t xb, int t, float inv_a, float (&s0v)[4]) {
+        uint8_t* rbp = bp + o_r;
         float e32[NH][16], e16[NH][8];
 #pragma unroll
         for (int h = 0; h < NH; ++h) {
@@ -410,33 +381,33 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
 #pragma unroll
                 for (int q = 0; q < 4; ++q) rr_v[h][rr][q] = valid ? fmaf(wl[q], inv_se, prm.alpha) * inv_den : 0.f;   // ref :380-383
             }
-        before_write();
 #pragma unroll
-            for (int h = 0; h < NH; ++h)
+        for (int h = 0; h < NH; ++h)
 #pragma unroll
-                for (int rr = 0; rr < 2; ++rr) {
-                    const int rt = h * 64 + 16 * warp + g8 + 8 * rr;     // row within the tile
-                    const uint32_t rbase = (uint32_t)(rt >> 6) * 4096u + (uint32_t)(rt & 7) * 2u;
-                    const int c16 = (rt & 63) >> 3;
+            for (int rr = 0; rr < 2; ++rr) {
+                const int rt = h * 64 + 16 * warp + g8 + 8 * rr;     // row within the tile
+                const uint32_t rbase = (uint32_t)(rt >> 6) * 4096u + (uint32_t)(rt & 7) * 2u;
+                const int c16 = (rt & 63) >> 3;
 #pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        const int k = 8 * (q >> 1) + 2 * t4 + (q & 1);
-                        if (k < K) {
-                            const float r = rr_v[h][rr][q];
-                            s0v[q] += r;
-                            const float rs = r * SR;
-                            const __half hh = __float2half_rn(rs);
-                            const uint32_t off = rbase + (uint32_t)k * 128u + (uint32_t)(((c16 ^ (k & 7)) & 7) << 4);
-                            *reinterpret_cast<__half*>(rbp + off) = hh;                                          // row k
-                            *reinterpret_cast<__half*>(rbp + off + 2048u) = __float2half_rn(rs - __half2float(hh));   // row 16 + k
-                        }
+                for (int q = 0; q < 4; ++q) {
+                    const int k = 8 * (q >> 1) + 2 * t4 + (q & 1);
+                    if (k < K) {
+                        const float r = rr_v[h][rr][q];
+                        s0v[q] += r;
+                        const float rs = r * SR;
+                        const __half hh = __float2half_rn(rs);
+                        const uint32_t off = rbase + (uint32_t)k * 128u + (uint32_t)(((c16 ^ (k & 7)) & 7) << 4);
+                        *reinterpret_cast<__half*>(rbp + off) = hh;                                          // row k
+                        *reinterpret_cast<__half*>(rbp + off + 2048u) = __float2half_rn(rs - __half2float(hh));   // row 16 + k
                     }
                 }
+            }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // R stores -> visible to the MMA (async proxy)
     };
     // statistics of one tile (warps SW0 .. SW0 + 3): S1 += X^T . [R hi ; R lo] (m64n32, A = X hi MN-major) and X lo^T . R hi
     // (m64n16), one m64 block per 64 d
-    auto stats_tile = [&](uint32_t xb, uint32_t rb, bool first) {
+    auto stats_tile = [&](uint32_t xb, bool first) {
+        const uint32_t rb = base + o_r;
         wg_fence();
 #pragma unroll
         for (int ks = 0; ks < TR / 16; ++ks) {
@@ -453,7 +424,7 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
         wg_wait0();
     };
 
-    auto load_tile = [&](int t) {                                    // issuer only (serial, D = 256): one tile, hi + lo, into the X buffer
+    auto load_tile = [&](int t) {                                    // issuer only (D = 256): one tile, hi + lo, into the X buffer
         mbar_expect_tx(bar_tma, 2 * X_BYTES);
         const int row0 = c * cap + t * TR;
 #pragma unroll
@@ -550,64 +521,8 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
 
         float s0v[4] = {0.f, 0.f, 0.f, 0.f};                          // warps 0-3: S0 of components 8 (q / 2) + 2 t4 + q % 2
         const float inv_a = 1.0f / (a_scale * SX);
-        uint32_t s1_base;                                             // the S1 hand-over of this loop
 
-        if constexpr (PIPE) {
-            // mbarriers: xfull[b] tile landed in buffer b | xfree[b] the statistics MMAs reading buffer b (and the R buffer
-            // they used) have retired | rfull[e] soft-max wrote R buffer e.  Global tile counter g: row-tile buffer g % 3,
-            // R buffer g & 1; every barrier completes exactly once per tile that uses its buffer, so its phase parity is
-            // (g / 3) & 1 resp. (g / 2) & 1.
-            auto XFULL = [&](uint32_t b) { return bar_tma + 8u * b; };
-            auto XFREE = [&](uint32_t b) { return bar_tma + 8u * (3 + b); };
-            auto RFULL = [&](uint32_t e) { return bar_tma + 8u * (8 + e); };
-            const uint32_t g0 = tile_ctr;
-            auto load_tile_p = [&](int t, uint32_t g) {              // issuer: tile t of this class -> buffer g % 3
-                const uint32_t b = g % 3u;
-                if (g >= 3) mbar_wait(XFREE(b), ((g - 3) / 3u) & 1u);   // the previous tile in this buffer has been consumed
-                mbar_expect_tx(XFULL(b), 2 * X_BYTES);
-                const int row0 = c * cap + t * TR;
-#pragma unroll
-                for (int ch = 0; ch < NCH; ++ch) {
-                    tma_load_2d(base + b * 2 * X_BYTES + o_xh + ch * CH_BYTES, &map_h, ch * 64, row0, XFULL(b));
-                    tma_load_2d(base + b * 2 * X_BYTES + o_xl + ch * CH_BYTES, &map_l, ch * 64, row0, XFULL(b));
-                }
-                MGP_PROF(g, 0);
-            };
-            if (warp >= 4) {
-                if (warp >= 5 && loop == 0) {                        // the absorbed inactive classes, before the first statistics
-                    for (int j = (int)blockIdx.x; j < ABSORB * n_active && n_active + j < prm.C; j += n_active)
-                        replay_inactive(prm.clist[n_active + j], 5, 3);
-                }
-                if (tid == ISSUER && loop == 0) load_tile_p(0, g0);  // (later loops: prefetched under the previous loop's tail)
-                for (int t = 0; t < ntiles; ++t) {
-                    const uint32_t g = g0 + t;
-                    if (tid == ISSUER && t + 1 < ntiles) load_tile_p(t + 1, g + 1);
-                    mbar_wait(XFULL(g % 3u), (g / 3u) & 1u);
-                    mbar_wait(RFULL(g & 1u), (g >> 1) & 1u);
-                    stats_tile(base + (g % 3u) * 2 * X_BYTES, base + o_r + (g & 1u) * 8192u, t == 0);
-                    if (tid == ISSUER) MGP_PROF(g, 5);
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(XFREE(g % 3u));
-                }
-                if (tid == ISSUER && loop + 1 < L) load_tile_p(0, g0 + ntiles);   // the next loop's first tile, under this loop's tail
-            } else {
-                for (int t = 0; t < ntiles; ++t) {
-                    const uint32_t g = g0 + t;
-                    mbar_wait(XFULL(g % 3u), (g / 3u) & 1u);
-                    if (tid == 0) MGP_PROF(g, 1);
-                    estep_tile(base + (g % 3u) * 2 * X_BYTES, bp + o_r + (g & 1u) * 8192u, t, inv_a, s0v, [&]() {
-                        if (t >= 2) mbar_wait(XFREE((g - 2) % 3u), ((g - 2) / 3u) & 1u);   // the MMAs that read this R buffer have retired
-                    });
-                    __syncwarp();
-                    if (tid == 0) MGP_PROF(g, 4);
-                    if (lane == 0) mbar_arrive(RFULL(g & 1u));
-                }
-                const uint32_t gl = g0 + ntiles - 1;                 // the last statistics MMAs of this loop
-                mbar_wait(XFREE(gl % 3u), (gl / 3u) & 1u);
-            }
-            tile_ctr += (uint32_t)ntiles;
-            s1_base = base + ((tile_ctr + 1u) % 3u) * 2 * X_BYTES;   // idle until the next loop's second tile
-        } else if constexpr (WG1) {
+        if constexpr (WG1) {
             // xfull[s]: a tile landed in slot s.  Tile g of the class's timeline (row tile g % ntiles of loop
             // g / ntiles) goes to slot g & 1, so xfull[s] completes once per tile in slot s: phase parity (g / 2) & 1.
             // Slot g & 1 takes tile g + 2 as soon as the statistics MMAs of tile g have retired.
@@ -632,47 +547,45 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
                 const uint32_t g = tile_ctr;
                 mbar_wait(bar_tma + 8u * (g & 1u), (g >> 1) & 1u);
                 if (tid == 0) MGP_PROF(g, 1);
-                estep_tile(xslot(g), bp + o_r, t, inv_a, s0v, []() {});
+                estep_tile(xslot(g), t, inv_a, s0v);
                 if (tid == 0) MGP_PROF(g, 4);
                 __syncthreads();                                     // every warp's R rows are stored and fenced
-                stats_tile(xslot(g), base + o_r, t == 0);
+                stats_tile(xslot(g), t == 0);
                 if (tid == 0) MGP_PROF(g, 5);
                 __syncthreads();                                     // every warp's statistics MMAs retired: slot and R free
                 if (tid == ISSUER && g + 2 < n_total) load_tile_r(g + 2);   // (a loop's last two: the next loop's first two)
             }
-            s1_base = base + o_s1;
         } else {
-        for (int t = 0; t < ntiles; ++t, ++tile_ctr) {
-            const uint32_t par = tile_ctr & 1u;
-            if (tid == ISSUER) {
-                if (!(t == 0 && loop > 0)) {                                 // (a loop's first tile was prefetched by the previous loop)
-                    if (tile_ctr > 0) mbar_wait(bar_s, (tile_ctr - 1) & 1u); // previous statistics MMAs have read X and R
-                    load_tile(t);
-                    MGP_PROF(tile_ctr, 0);
+            for (int t = 0; t < ntiles; ++t, ++tile_ctr) {
+                const uint32_t par = tile_ctr & 1u;
+                if (tid == ISSUER) {
+                    if (!(t == 0 && loop > 0)) {                             // (a loop's first tile was prefetched by the previous loop)
+                        if (tile_ctr > 0) mbar_wait(bar_s, (tile_ctr - 1) & 1u);   // previous statistics MMAs have read X and R
+                        load_tile(t);
+                        MGP_PROF(tile_ctr, 0);
+                    }
+                }
+                if (warp < 4) {
+                    mbar_wait(bar_tma, par);
+                    if (tid == 0) MGP_PROF(tile_ctr, 1);
+                    estep_tile(base, t, inv_a, s0v);
+                    if (tid == 0) MGP_PROF(tile_ctr, 4);
+                }
+                __syncthreads();
+                if (warp >= 4) {
+                    mbar_wait(bar_tma, par);                                 // (the tile is visible to this warpgroup's MMAs)
+                    stats_tile(base, t == 0);
+                    if (tid == ISSUER) MGP_PROF(tile_ctr, 5);
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(bar_s);
                 }
             }
-            if (warp < 4) {
-                mbar_wait(bar_tma, par);
-                if (tid == 0) MGP_PROF(tile_ctr, 1);
-                estep_tile(base, bp + o_r, t, inv_a, s0v, []() {});
-                if (tid == 0) MGP_PROF(tile_ctr, 4);
+            if (tid == ISSUER && loop + 1 < L) {      // the next loop starts on the same rows: fetch its first tile under the tail
+                mbar_wait(bar_s, (tile_ctr - 1) & 1u);
+                load_tile(0);
             }
-            __syncthreads();
-            if (warp >= 4) {
-                mbar_wait(bar_tma, par);                                     // (the tile is visible to this warpgroup's MMAs)
-                stats_tile(base, base + o_r, t == 0);
-                if (tid == ISSUER) MGP_PROF(tile_ctr, 5);
-                __syncwarp();
-                if (lane == 0) mbar_arrive(bar_s);
-            }
+            mbar_wait(bar_s, (tile_ctr - 1) & 1u);                    // all statistics MMAs of this loop have retired
         }
-        if (tid == ISSUER && loop + 1 < L) {          // the next loop starts on the same rows: fetch its first tile under the tail
-            mbar_wait(bar_s, (tile_ctr - 1) & 1u);
-            load_tile(0);
-        }
-        mbar_wait(bar_s, (tile_ctr - 1) & 1u);                        // all statistics MMAs of this loop have retired
-        s1_base = base + o_s1;
-        }   // !PIPE
         if (tid == 0) MGP_PROF(tile_ctr - 1, 6);
         // ---- S0 over the class (warps 0-3: reduce over the 8 rows of a fragment column, then lanes 0-3 hold all 16)
         if (warp < 4) {
@@ -686,7 +599,7 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
             }
         }
         // ---- S1 from the statistics warpgroup's registers to the owners: s1[d][k] = (hi.hi + lo.hi) + hi.lo
-        float* s_s1 = reinterpret_cast<float*>(bp + (s1_base - base));
+        float* s_s1 = reinterpret_cast<float*>(bp + o_s1);
         if (warp >= SW0) {
 #pragma unroll
             for (int mb = 0; mb < MB; ++mb)
@@ -706,7 +619,6 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
 #pragma unroll
             for (int k = 0; k < KT; ++k) sacc[k] = s_s1[tid * S1_STRIDE + k];
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // PIPE: the hand-over area is a TMA destination again
         __syncthreads();
         // ---- gradient + diversity + Adam on the owned elements (ref model.py:385-397; SURVEY KA6)
         if (own) {
@@ -752,16 +664,15 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
 }
 
 template <int D>
-size_t em_tc_smem(int kt, bool pipe) {
-    const size_t tr = em_rows(D, pipe), nx = pipe ? 3 : (em_one_wg(D, pipe) ? 2 : 1);
-    return 1024 + nx * 2 * (size_t)(D / 64) * tr * 128 + (size_t)(D / 64) * 4096 + (pipe ? 2 : 1) * (tr / 64) * 4096 +
-           (pipe ? 0 : (size_t)((D * S1_STRIDE * 4 + 15) & ~15)) +
+size_t em_tc_smem(int kt) {
+    const size_t tr = em_rows(D), nx = em_one_wg(D) ? 2 : 1;
+    return 1024 + nx * 2 * (size_t)(D / 64) * tr * 128 + (size_t)(D / 64) * 4096 + (tr / 64) * 4096 +
+           (size_t)((D * S1_STRIDE * 4 + 15) & ~15) +
            ((size_t)kt * kt + 136 + 6 * 16 + 8 + 8 * (size_t)(32 * ((kt * (kt - 1) / 2 + kt + 31) / 32))) * 4 + 128;
 }
 
 }  // namespace
 
-int mgp_opt_em_pipe();   // abi.cu
 static long long* g_em_tc_prof = nullptr;
 static int g_em_tc_prof_class = 0;
 void mgp_em_tc_set_prof(void* p, int cls) { g_em_tc_prof = reinterpret_cast<long long*>(p); g_em_tc_prof_class = cls; }
@@ -774,10 +685,9 @@ int mgp_em_tc_launch(const void* shadow_h, const void* shadow_l, const float* sh
                      const int32_t* sched, float* mu, const float* sigma, float* weight, float* exp_avg, float* exp_avg_sq,
                      int* status, int num_em_loop, float alpha, double lr, double beta1, double beta2, double adam_eps,
                      double tau, float lamda, int C, int K, int D, int cap, cudaStream_t st) {
-    CUtensorMap mh, ml, mh1, ml1;                   // 128-row boxes; 64-row boxes for the one-warpgroup kernel (D = 128)
+    CUtensorMap mh, ml;                             // boxes of em_rows(D) rows: one tile, hi and lo
     const uint64_t rows = (uint64_t)C * cap;
-    if (!make_map_f16(&mh, shadow_h, rows, D, 128) || !make_map_f16(&ml, shadow_l, rows, D, 128)) return MGP_ERR_UNSUPPORTED;
-    if (D == 128 && (!make_map_f16(&mh1, shadow_h, rows, D, 64) || !make_map_f16(&ml1, shadow_l, rows, D, 64)))
+    if (!make_map_f16(&mh, shadow_h, rows, D, em_rows(D)) || !make_map_f16(&ml, shadow_l, rows, D, em_rows(D)))
         return MGP_ERR_UNSUPPORTED;
     EmTcParams prm;
     prm.xx = shadow_xx; prm.bc = bias_corr; prm.order = order; prm.sched = sched; prm.mu = mu; prm.sigma = sigma; prm.weight = weight;
@@ -787,33 +697,20 @@ int mgp_em_tc_launch(const void* shadow_h, const void* shadow_l, const float* sh
     prm.num_em_loop = num_em_loop; prm.C = C; prm.K = K; prm.cap = cap;
     prm.prof = g_em_tc_prof; prm.prof_class = g_em_tc_prof_class;
     prm.clist = reinterpret_cast<const int32_t*>(bias_corr + (size_t)5 * num_em_loop * C + 4);
-    const bool pipe = mgp_opt_em_pipe() != 0 && D == 128;
-    static int n_sm = 0;
-    if (n_sm == 0) {
-        int devi = 0;
-        MGP_CUDA(cudaGetDevice(&devi));
-        MGP_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, devi));
-    }
-    prm.pipe_max = pipe ? n_sm : 0;
-#define MGP_EMTC(DD, KK, PP, MH, ML)                                                                                \
+#define MGP_EMTC(DD, KK)                                                                                            \
     do {                                                                                                            \
-        const size_t smem = em_tc_smem<DD>(KK, PP);                                                                 \
-        MGP_CUDA(cudaFuncSetAttribute(em_tc_kernel<DD, KK, PP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        em_tc_kernel<DD, KK, PP><<<C, em_threads(DD, PP), smem, st>>>(MH, ML, prm);                                 \
+        const size_t smem = em_tc_smem<DD>(KK);                                                                     \
+        MGP_CUDA(cudaFuncSetAttribute(em_tc_kernel<DD, KK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+        em_tc_kernel<DD, KK><<<C, em_threads(DD), smem, st>>>(mh, ml, prm);                                         \
     } while (0)
-#define MGP_EMTC_K(DD, PP, MH, ML)                                                                                  \
+#define MGP_EMTC_K(DD)                                                                                              \
     do {                                                                                                            \
-        if (K <= 5) MGP_EMTC(DD, 5, PP, MH, ML);                                                                    \
-        else if (K <= 10) MGP_EMTC(DD, 10, PP, MH, ML);                                                             \
-        else MGP_EMTC(DD, 16, PP, MH, ML);                                                                          \
+        if (K <= 5) MGP_EMTC(DD, 5);                                                                                \
+        else if (K <= 10) MGP_EMTC(DD, 10);                                                                         \
+        else MGP_EMTC(DD, 16);                                                                                      \
     } while (0)
-    if (D == 128) {
-        if (pipe) MGP_EMTC_K(128, true, mh, ml);
-        MGP_CHECK_LAUNCH();
-        MGP_EMTC_K(128, false, mh1, ml1);            // one warpgroup (returns at once when the pipelined kernel took the call)
-    } else {
-        MGP_EMTC_K(256, false, mh, ml);
-    }
+    if (D == 128) MGP_EMTC_K(128);
+    else MGP_EMTC_K(256);
 #undef MGP_EMTC_K
 #undef MGP_EMTC
     MGP_CHECK_LAUNCH();

@@ -184,13 +184,13 @@ def test_headline_head_vs_fp64_oracle_batch16():
 
 
 # ------------------------------------------------------------------------------------------------ EM
-# (em_tc, em_fused, em_pipe) switches of mgp_set_option
-EM_PATHS = {"tc": (1, 1, 1), "tc_serial": (1, 1, 0), "fused": (0, 1, 1), "multilaunch": (0, 0, 1)}
+# (em_tc, em_fused) switches of mgp_set_option
+EM_PATHS = {"tc": (1, 1), "fused": (0, 1), "multilaunch": (0, 0)}
 
 
 class em_path:
-    """Select which update_GMM implementation the library takes: tensor-core kernel (csrc/em_tc.cu; pipelined, or one
-    tile at a time), fp32 cluster kernel, or the multi-launch path (identical semantics; the tests cross-check them)."""
+    """Select which update_GMM implementation the library takes: tensor-core kernel (csrc/em_tc.cu), fp32 cluster
+    kernel, or the multi-launch path (identical semantics; the tests cross-check them)."""
 
     def __init__(self, name):
         self.want = EM_PATHS[name]
@@ -198,15 +198,13 @@ class em_path:
     def __enter__(self):
         from mgproto_b200 import _lib
         lib = _lib.load()
-        self.prev = (lib.mgp_set_option(b"em_tc", self.want[0]), lib.mgp_set_option(b"em_fused", self.want[1]),
-                     lib.mgp_set_option(b"em_pipe", self.want[2]))
+        self.prev = (lib.mgp_set_option(b"em_tc", self.want[0]), lib.mgp_set_option(b"em_fused", self.want[1]))
 
     def __exit__(self, *a):
         from mgproto_b200 import _lib
         lib = _lib.load()
         lib.mgp_set_option(b"em_tc", self.prev[0])
         lib.mgp_set_option(b"em_fused", self.prev[1])
-        lib.mgp_set_option(b"em_pipe", self.prev[2])
 
 
 def _run_em(g, math, path):
@@ -233,7 +231,7 @@ def _run_em(g, math, path):
     return net, outs
 
 
-@pytest.mark.parametrize("path", ["tc", "tc_serial", "fused", "multilaunch"])
+@pytest.mark.parametrize("path", ["tc", "fused", "multilaunch"])
 @pytest.mark.parametrize("math", ["auto", "fp32"])
 def test_headline_update_gmm_vs_reference(hl, math, path):
     """Two update_GMM calls (156 + 137 active classes, 5 flagged-but-short classes, Adam at step 1000) after the
@@ -299,7 +297,7 @@ def test_variant_shapes_head_and_em_vs_fp64_oracle(C, K, D, sigma_mode):
     adam = O.AdamOracle((C, K, D), lr=3e-3)
     adam.m, adam.v, adam.t = f64(am), f64(av), step0
     mu_ref, wt_ref, _ = O.update_gmm(bank, flags[0], f64(mu), f64(sg), f64(wt), adam)
-    for path in ("tc", "tc_serial", "multilaunch"):           # (tc falls through to the fp32 kernels where it does not apply)
+    for path in ("tc", "multilaunch"):                        # (tc falls through to the fp32 kernels where it does not apply)
         net = _net(C, K, D, T, cap, mu, sg, wt, "auto")
         _fill_bank(net, rows, short, cap - 11)
         _seed_adam(net, am, av, step0)

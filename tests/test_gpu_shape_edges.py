@@ -14,10 +14,9 @@ Reference: the float64 oracle (oracle/mgproto_oracle.py) or a float64 torch rest
 the gradient is routed through the kernel's own picks (O.head_backward(..., idx=...), pick deviation < 1e-4).
 
 Each case runs under torch.profiler (CUDA activity) and asserts that the instantiations COVERS assigns to it were
-launched.  Two choices are made on the device, and there a trace entry proves only the launch: the pipelined vs the
-one-warpgroup EM kernel (both are launched at D = 128; the one that does not apply returns at once), and the image-tile
-vs the 128-patch-tile top-1 kernel when the host does not know sigma is isotropic.  Those cases select the kernel that
-does the work with the em_pipe switch and with staging, as the existing tests do.
+launched.  One choice is made on the device, and there a trace entry proves only the launch: the image-tile vs the
+128-patch-tile top-1 kernel when the host does not know sigma is isotropic.  Those cases select the kernel that does
+the work with staging, as the existing tests do.
 
 tests/test_kernel_coverage_cpu.py checks, without a GPU, that every template instantiation in the built library is a
 key of COVERS or is listed in its EXEMPT."""
@@ -76,15 +75,12 @@ COVERS = {
     "logprob_simt_kernel<0>": _E + "test_head_large_maps[21x21-d128]",
     "logprob_simt_kernel<1>": _E + "test_head_large_maps[21x21-d128]",
     "logprob_simt_kernel<2>": _E + "test_head_large_maps[21x21-d128]",
-    "em_tc_kernel<128, 5, true>": _E + "test_em_instantiations[k5-d128-cap64-tc]",
-    "em_tc_kernel<128, 5, false>": _E + "test_em_instantiations[k2-d128-cap37-tc_serial]",
-    "em_tc_kernel<128, 10, true>": _E + "test_em_instantiations[k7-d128-cap65-tc]",
-    "em_tc_kernel<128, 10, false>": _E + "test_em_instantiations[k7-d128-cap65-tc_serial]",
-    "em_tc_kernel<128, 16, true>": _E + "test_em_instantiations[k16-d128-cap1000-tc]",
-    "em_tc_kernel<128, 16, false>": _E + "test_em_instantiations[k11-d128-cap200-tc_serial]",
-    "em_tc_kernel<256, 5, false>": _E + "test_em_instantiations[k3-d256-cap50-tc]",
-    "em_tc_kernel<256, 10, false>": _E + "test_em_instantiations[k10-d256-cap64-tc]",
-    "em_tc_kernel<256, 16, false>": _E + "test_em_instantiations[k16-d256-cap129-tc_serial]",
+    "em_tc_kernel<128, 5>": _E + "test_em_instantiations[k2-d128-cap37-tc]",
+    "em_tc_kernel<128, 10>": _E + "test_em_instantiations[k7-d128-cap65-tc]",
+    "em_tc_kernel<128, 16>": _E + "test_em_instantiations[k11-d128-cap200-tc]",
+    "em_tc_kernel<256, 5>": _E + "test_em_instantiations[k3-d256-cap50-tc]",
+    "em_tc_kernel<256, 10>": _E + "test_em_instantiations[k10-d256-cap64-tc]",
+    "em_tc_kernel<256, 16>": _E + "test_em_instantiations[k16-d256-cap129-tc]",
     "em_fused_kernel<128, 3>": _E + "test_em_instantiations[k2-d128-cap37-fused]",
     "em_fused_kernel<128, 5>": _E + "test_em_instantiations[k7-d128-cap65-fused]",
     "em_fused_kernel<128, 8>": _E + "test_em_instantiations[k16-d128-cap8-fused]",
@@ -370,18 +366,22 @@ def test_out_of_range_shapes_are_refused():
 EM_CASES = [(2, 128, 37), (5, 128, 64), (5, 128, 1000), (7, 128, 65), (11, 128, 200), (16, 128, 8), (16, 128, 1000),
             (3, 256, 50), (5, 256, 200), (10, 256, 64), (16, 256, 129), (1, 128, 50),
             (2, 64, 37), (10, 64, 65), (16, 64, 200)]
-EM_RUNS = [(K, D, cap, path) for K, D, cap in EM_CASES
-           for path in {64: ("fused",), 128: ("tc", "tc_serial", "fused"), 256: ("tc", "tc_serial")}[D]]
+# every case also runs sparse: a random quarter, then half, of the classes flagged, so that most blocks only replay
+# the others' Adam steps and, in the tensor-core kernel at D = 128 (active classes first), run classes far from their
+# own index
+EM_RUNS = [(K, D, cap, path, sparse) for K, D, cap in EM_CASES
+           for path in {64: ("fused",), 128: ("tc", "fused"), 256: ("tc",)}[D] for sparse in (False, True)]
 
 
 @functools.lru_cache(maxsize=None)
-def _em_case(K, D, cap):
+def _em_case(K, D, cap, sparse=False):
     """Seeded inputs and the float64 oracle's two successive update_GMM calls (ref model.py:277-301)."""
     from oracle import mgproto_oracle as O
     C = 40 if cap < 1000 else 12
     mu, sg, wt = HC.mixture(C, K, D, seed=600 + K + D + cap)
     rows = HC.bank_rows(C, K, D, cap, mu, seed=601 + cap)
-    am, av, flags, short, step0 = HC.em_state(C, K, D, seed=602 + K, n_active=(C, C - 7), n_short=2, step0=500)
+    n_active = (C // 4, C // 2) if sparse else (C, C - 7)
+    am, av, flags, short, step0 = HC.em_state(C, K, D, seed=602 + K, n_active=n_active, n_short=2, step0=500)
     short_len = cap // 2
     bank = O.MemoryBankOracle(C, D, cap, dtype=np.float64)
     bank.data[:] = rows
@@ -397,11 +397,13 @@ def _em_case(K, D, cap):
                 step0=step0, ref=ref, adam=(adam.m, adam.v, adam.t))
 
 
-@pytest.mark.parametrize("K,D,cap,path", EM_RUNS, ids=["k%d-d%d-cap%d-%s" % r for r in EM_RUNS])
-def test_em_instantiations(request, K, D, cap, path):
-    """Two update_GMM calls (all classes flagged, then all but 7; two classes short; Adam at step 500): mu (whole and
-    per class), the movement, pi, both Adam moments and the step count against the float64 oracle."""
-    g = _em_case(K, D, cap)
+@pytest.mark.parametrize("K,D,cap,path,sparse", EM_RUNS,
+                         ids=["k%d-d%d-cap%d-%s" % r[:4] + ("-sparse" if r[4] else "") for r in EM_RUNS])
+def test_em_instantiations(request, K, D, cap, path, sparse):
+    """Two update_GMM calls (all classes flagged, then all but 7, or sparse: a quarter, then half; two classes short;
+    Adam at step 500): mu (whole and per class), the movement, pi, both Adam moments and the step count against the
+    float64 oracle."""
+    g = _em_case(K, D, cap, sparse)
     C = g["C"]
     net = _net(C, K, D, 20, cap, g["mu"], g["sg"], g["wt"], "auto")
     _fill_bank(net, g["rows"], g["short"], g["short_len"])

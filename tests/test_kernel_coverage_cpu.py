@@ -37,8 +37,8 @@ def _instantiations():
 def test_kernel_key_normalises_both_demanglers():
     assert E.kernel_key("void <unnamed>::head_top1_kernel<(int)32, (int)1, (int)256>(const unsigned long long *, int)") \
         == "head_top1_kernel<32, 1, 256>"
-    assert E.kernel_key("void (anonymous namespace)::em_tc_kernel<128, 16, false>(CUtensorMap_st, "
-                        "(anonymous namespace)::EmTcParams)") == "em_tc_kernel<128, 16, false>"
+    assert E.kernel_key("void (anonymous namespace)::em_tc_kernel<128, 16>(CUtensorMap_st, "
+                        "(anonymous namespace)::EmTcParams)") == "em_tc_kernel<128, 16>"
     assert E.kernel_key("void <unnamed>::normalize_fwd_kernel<__nv_bfloat16, (bool)1>(const T1 *, float *)") \
         == "normalize_fwd_kernel<__nv_bfloat16, true>"
     assert E.kernel_key("<unnamed>::proto_weight_kernel(const float *, int)") == "proto_weight_kernel"

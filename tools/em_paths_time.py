@@ -1,12 +1,16 @@
 #!/usr/bin/env python
 """Time update_GMM (cfg2 / cfg3 mixture shapes) through each implementation: tensor-core kernel, fp32 cluster kernel,
-multi-launch path, at 80 .. 200 active classes.  At D = 128 the tensor-core kernel takes its pipelined variant while
-the active classes fit one CTA per SM (132 on an H100 SXM) and its one-warpgroup variant (two CTAs per SM) beyond;
-tc_serial always takes the latter.  CUDA events, 20 calls after 3 warm-ups; prints the card and its power limit."""
+multi-launch path, at 1 .. 200 active classes.  The active classes are a seeded random set (the seed is their count,
+as in tests/test_gpu_em_waves.py), as in training, where any class can be flagged.  CUDA events, 20 calls after 3
+warm-ups; prints the card and its power limit.
+
+    python tools/em_paths_time.py [--paths tc,fused,multilaunch] [--dims 128,256]"""
+import argparse
 import os
 import subprocess
 import sys
 
+import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -14,26 +18,35 @@ sys.path.insert(0, ROOT)
 import bench                                   # noqa: E402
 from mgproto_b200 import _lib                  # noqa: E402
 
+PATHS = {"tc": (1, 1), "fused": (0, 1), "multilaunch": (0, 0)}    # (em_tc, em_fused) switches of mgp_set_option
+COUNTS = (1, 8, 40, 80, 100, 132, 133, 146, 200)
+
+ap = argparse.ArgumentParser()
+ap.add_argument("--paths", default="tc,fused,multilaunch")
+ap.add_argument("--dims", default="128,256")
+args = ap.parse_args()
 dev = torch.device("cuda:0")
 torch.cuda.set_device(0)
 lib = _lib.load()
 card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
                       stdout=subprocess.PIPE, text=True).stdout.strip()
 print("card: %s, %d SMs" % (card, torch.cuda.get_device_properties(0).multi_processor_count))
-for D in (128, 256):
+for D in (int(d) for d in args.dims.split(",")):
     bench.CFG["D"] = D
     net = bench.build_model(dev)
+    C = net.queue.updated.numel()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    for name, (tc, fused, pipe) in (("tc", (1, 1, 1)), ("tc_serial", (1, 1, 0)), ("fused", (0, 1, 1)), ("multilaunch", (0, 0, 1))):
-        if D == 256 and name == "tc_serial":
-            continue
+    for name in args.paths.split(","):
+        tc, fused = PATHS[name]
         lib.mgp_set_option(b"em_tc", tc)
         lib.mgp_set_option(b"em_fused", fused)
-        lib.mgp_set_option(b"em_pipe", pipe)
-        for n_act in (80, 132, 133, 146, 200):
+        for n_act in COUNTS:
+            flags = torch.zeros(C, dtype=torch.uint8)
+            flags[np.random.default_rng(n_act).permutation(C)[:n_act]] = 1
+            flags = flags.to(dev)
+
             def run():
-                net.queue.updated.zero_()
-                net.queue.updated[:n_act] = 1
+                net.queue.updated.copy_(flags)
                 net.update_GMM()
             for _ in range(3):
                 run()
@@ -44,7 +57,7 @@ for D in (128, 256):
                 run()
             e1.record()
             torch.cuda.synchronize()
-            print("D=%d %-12s active=%3d  %.1f us per update_GMM (incl. 2 tiny fills)" % (D, name, n_act, e0.elapsed_time(e1) / 20 * 1e3))
+            print("D=%d %-12s active=%3d  %.1f us per update_GMM (incl. 1 tiny copy)" % (D, name, n_act, e0.elapsed_time(e1) / 20 * 1e3))
     lib.mgp_set_option(b"em_tc", 1)
     lib.mgp_set_option(b"em_fused", 1)
     net.sync_optimizer_state()

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Where the tensor-core EM kernel (csrc/em_tc.cu) spends a class's timeline: clock64 stamps of its pipeline phases for
-one class, printed per row tile (128 rows; 64 in the one-warpgroup variant) in microseconds at the SM clock read
-from nvidia-smi."""
+one class, printed per row tile (64 rows at D = 128, 128 at D = 256) in microseconds at the SM clock read from
+nvidia-smi."""
 import os
 import subprocess
 import sys
@@ -18,10 +18,9 @@ torch.cuda.set_device(0)
 lib = _lib.load()
 net = bench.build_model(dev)
 buf = torch.zeros(64 * 8, dtype=torch.int64, device=dev)
-# <= #SMs (132 on an H100 SXM): the pipelined kernel, where the stamped CTA index is the rank among the active classes;
-# above: the one-warpgroup kernel, where it is the class index
+# classes [:N_ACT] are active; the kernel stamps the CTA that runs class `cls` (the first and the last active class)
 N_ACT = int(os.environ.get("N_ACT", "120"))
-for cls in (3, 120):
+for cls in (0, N_ACT - 1):
     for _ in range(3):
         net.queue.updated.fill_(1)
         net.queue.updated[N_ACT:] = 0
