@@ -138,6 +138,23 @@ int mgp_logprob_fwd(const float* xhat_nd, const float* mu, const float* sigma, f
                     float eps_log, float* out, int out_layout, int B, int HW, int P, int D,
                     int math, void* ws, size_t ws_bytes, void* stream);
 
+/* ---- a14 over feature maps: per-patch class log-densities -----------------------------------
+ * ref: model.py:403-421 (_score, as_average=False), :323-336 (_estimate_log_prob, eps = 1e-10 in
+ * (sigma+eps) and log(sigma+eps)), train_and_test.py:199 (sum_c p(x|c)).  For every patch n = b*HW + hw of
+ * xhat_nd [N,D] (normalised rows, ref model.py:210-211) and every class c:
+ *   out_bchw[(b*C + c)*HW + hw] = logsumexp_k( log p_ck(x_n) + log(pi_ck + 1e-10) )   ([B,C,HW], fp32)
+ *   out_bhw[b*HW + hw]          = logsumexp_c out_bchw[...]                           ([B,HW]; may be NULL)
+ * mu/sigma [P,D] (P = C*K, class-major), weight_cp = last_layer.weight [C,P]: pi_ck = weight_cp[c, c*K + k].
+ * MGP_MATH_TC_ISO (the caller asserts sigma constant over d inside every prototype), D in {64, 128}, K <= 64:
+ * one tensor-core kernel, the [N,P] log-likelihood never reaches HBM; MGP_MATH_TC_ISO_REUSE: the same with the
+ * prototype-side operands of `ws` kept from the previous call with unchanged mu / sigma.  A false assertion yields
+ * NaN outputs.  Every other math mode and shape: mgp_logprob_fwd into row chunks of `ws`, then a log-sum-exp
+ * kernel.  No limit on HW; N < 2^31.  ws: mgp_log_density_ws_bytes(B, HW, C, K, D, math) bytes. */
+size_t mgp_log_density_ws_bytes(int B, int HW, int C, int K, int D, int math);
+int mgp_log_density(const float* xhat_nd, const float* mu, const float* sigma, const float* weight_cp,
+                    float* out_bchw, float* out_bhw, int B, int HW, int C, int K, int D, int math,
+                    void* ws, size_t ws_bytes, void* stream);
+
 /* ---- a4-a7  top-T mining + mixture logits ------------------------------------------------
  * ref: model.py:188-206 (global_max_pooling_gmm_topT), :214-222, :254, NonNegLinear :54-74.
  * logp_bphw [B,P,HW] (MGP_OUT_LOGP_BPHW).  Per (b,p): the T largest over HW, descending

@@ -33,6 +33,8 @@ SIGNATURES = {
     "mgp_normalize_bwd_x": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "mgp_logprob_ws_is_prototype_only": (_i, [_i, _i, _i, _i]),
     "mgp_logprob_fwd": (_i, [_vp, _vp, _vp, _f, _f, _vp, _i, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
+    "mgp_log_density_ws_bytes": (_sz, [_i] * 6),
+    "mgp_log_density": (_i, [_vp] * 6 + [_i] * 6 + [_vp, _sz, _vp]),
     "mgp_head_select": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "mgp_head_select_np": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "mgp_head_select_top1": (_i, [_vp] * 9 + [_i] * 6 + [_vp]),

@@ -786,6 +786,28 @@ bool mgp_logprob_tc_stage_ptrs(void* ws, size_t ws_bytes, long long N, int P, in
     return true;
 }
 
+// The prototype pre-pass alone (run != 0; else the operands are already there), into the prototype slots of a workspace
+// of mgp_logprob_tc_ws_bytes(0, P, D) bytes or more; returns where they are (log_density.cu reads them)
+int mgp_logprob_tc_proto_prep(const float* mu, const float* sigma, float eps, float eps_log, void* ws, int P, int D,
+                              int run, void** bh, void** bl, float** e0, float** e1, float** e2, int** flag,
+                              cudaStream_t st) {
+    const WsLayout w = ws_layout(0, P, D);
+    uint8_t* wsb = reinterpret_cast<uint8_t*>(ws);
+    *bh = wsb + w.bh;
+    *bl = wsb + w.bl;
+    *e0 = reinterpret_cast<float*>(wsb + w.e0);
+    *e1 = reinterpret_cast<float*>(wsb + w.e1);
+    *e2 = reinterpret_cast<float*>(wsb + w.e2);
+    *flag = reinterpret_cast<int*>(wsb + w.flag);
+    if (run) {
+        MGP_CUDA(cudaMemsetAsync(*flag, 0, 4, st));
+        tc_proto_prep_kernel<<<(P + 7) / 8, 256, 0, st>>>(mu, sigma, eps, eps_log, reinterpret_cast<__half*>(*bh),
+                                                          reinterpret_cast<__half*>(*bl), *e0, *e1, *e2, *flag, P, D);
+        MGP_CHECK_LAUNCH();
+    }
+    return MGP_OK;
+}
+
 int mgp_logprob_tc_launch(const float* xhat, const float* mu, const float* sigma, float eps, float eps_log, float* out,
                           int layout, int B, int HW, int P, int D, void* ws, size_t ws_bytes, int reuse_operands,
                           int assume_iso, int x_staged, cudaStream_t st) {

@@ -193,6 +193,21 @@ class MGProto(nn.Module):
         (train_and_test.py:182-199), without mining the other T-1 levels or materialising log p."""
         return ops.head_level0(x_add, self.prototype_means, self.prototype_covs, self.last_layer.weight, self.math_mode)
 
+    @torch.no_grad()
+    def log_density_maps(self, x_add):
+        """Per-patch class log-densities of the add-on features x_add [B,D,H,W] (fp32 / bf16 / fp16, NCHW or
+        channels_last), normalised as the head does (ref model.py:210): -> (logp_c [B,C,H,W], logp_all [B,H,W]), fp32.
+        logp_c[b,c,h,w] = _score(x_hat[b,:,h,w], mu_c, sigma_c, pi_c, as_average=False) (ref model.py:403-421, eps =
+        1e-10), pi from last_layer.weight's class-diagonal blocks; logp_all = logsumexp over the classes, the per-patch
+        form of the OoD statistic sum_c p(x|c) (ref train_and_test.py:199).  No gradient."""
+        C, K, D = self.prototype_means.shape
+        B, _, H, W = x_add.shape
+        xhat, _, _ = ops.normalize_fwd(x_add.detach())
+        lc, la = ops.log_density(xhat, self.prototype_means.detach().reshape(C * K, D),
+                                 self.prototype_covs.detach().reshape(C * K, D), self.last_layer.weight.detach(),
+                                 B, H * W, C, K, math=self.math_mode)
+        return lc.view(B, C, H, W), la.view(B, H, W)
+
     def forward(self, x, gt):
         """ref model.py:208-254 -> (log_probs [B,C,T], x_embed [B,sz_embedding])."""
         x_add, x_embed = self.conv_features(x)

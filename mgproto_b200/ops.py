@@ -18,7 +18,7 @@ from ._lib import (MGP_MATH_AUTO, MGP_MATH_FP32, MGP_MATH_TC, MGP_MATH_TC_ISO, M
                    MGP_OUT_LOGP_NP, MGP_OUT_NEGP_BPHW, MGP_OUT_TOP1_BP, MGP_X_BF16, MGP_X_F16, MGP_X_F32, MGP_X_NHWC,
                    check)
 
-__all__ = ["normalize_fwd", "logprob", "logprob_top1", "head_select", "head_select_top1", "head_level0", "head_forward", "HeadFunction", "mined_gather", "bank_enqueue",
+__all__ = ["normalize_fwd", "logprob", "log_density", "logprob_top1", "head_select", "head_select_top1", "head_level0", "head_forward", "HeadFunction", "mined_gather", "bank_enqueue",
            "bank_linearize", "bank_shadow_sync", "em_plan", "em_stats", "em_update", "update_gmm", "em_estep", "em_mstep_closed", "em_mstep_div", "topt_pool", "ood_score", "push_argmin", "push_argmin_top1", "mine_cross_entropy",
            "MATH_MODES"]
 
@@ -35,14 +35,15 @@ def sigma_is_isotropic(sigma: torch.Tensor) -> bool:
     """True if sigma is constant over the feature dim inside every prototype.  One tiny device reduction + host
     read, cached per (storage, version): sigma never changes in the reference's training loop."""
     # ([C,K,D] and its [P,D] view are the same question: the key leaves the leading shape out)
+    # (an entry keeps its tensor alive: a freed tensor's address and version 0 could otherwise come back with other values)
     key = (sigma.data_ptr(), sigma._version, sigma.numel(), sigma.shape[-1], str(sigma.device))
     hit = _iso_cache.get(key)
     if hit is None:
-        hit = bool((sigma == sigma[..., :1]).all().item())
+        hit = (bool((sigma == sigma[..., :1]).all().item()), sigma)
         if len(_iso_cache) >= 8:
             _iso_cache.clear()
         _iso_cache[key] = hit
-    return hit
+    return hit[0]
 
 _launches = 0          # kernels launched through this module (bench.py reports it as gpu_launches)
 
@@ -249,6 +250,58 @@ def logprob(xhat_nd, mu_pd, sigma_pd, layout=MGP_OUT_LOGP_NP, B=None, HW=None, e
             _PROTO_OPERANDS.popitem(last=False)
     _count(1 if m in (MGP_MATH_TC_REUSE, MGP_MATH_TC_ISO_REUSE) else (3 if nbytes > (P * D + P) * 4 else 2))
     return (out, ws) if return_ws else out
+
+
+_DENSITY_OPERANDS = collections.OrderedDict()   # as _PROTO_OPERANDS, for log_density's tensor-core workspace
+
+
+@_on_device
+def log_density(xhat_nd, mu_pd, sigma_pd, weight_cp, B, HW, C, K, math="auto", want_all=True):
+    """ref model.py:403-421 (_score, as_average=False) for every patch and class: xhat [N,D] (N = B*HW normalised
+    rows), mu/sigma [P,D], last_layer.weight [C,P] -> (logp_c [B,C,HW], logp_all [B,HW] | None), fp32, where
+    logp_c = logsumexp_k(log p_ck + log(pi_ck + 1e-10)) and logp_all = logsumexp_c logp_c.  No gradient.
+    Isotropic sigma, D in {64, 128} and K <= 64 run the tensor-core kernel (math "auto", "tc" or "tc_iso"); while mu
+    and sigma are unchanged its prototype operands are kept between calls.  Everything else runs mgp_logprob_fwd in
+    row chunks under `math` and a log-sum-exp kernel."""
+    x = _req(xhat_nd, torch.float32, "xhat")
+    mu = _req(mu_pd, torch.float32, "mu")
+    sg = _req(sigma_pd, torch.float32, "sigma")
+    w = _req(weight_cp, torch.float32, "last_layer.weight")
+    N, D = x.shape
+    P = C * K
+    if B * HW != N or mu.shape != (P, D) or sg.shape != (P, D) or w.shape != (C, P):
+        raise RuntimeError("mgproto_b200: shape mismatch in log_density")
+    lib = _lib.load()
+    m = _math(math)
+    if m not in (MGP_MATH_FP32, MGP_MATH_TC, MGP_MATH_AUTO, MGP_MATH_TC_ISO):
+        raise RuntimeError("mgproto_b200: log_density takes math 'auto', 'fp32', 'tc' or 'tc_iso'")
+    if m != MGP_MATH_FP32:
+        iso = sigma_is_isotropic(sg)
+        if m == MGP_MATH_TC_ISO and not iso:
+            raise RuntimeError("mgproto_b200: math 'tc_iso' needs sigma constant over d inside every prototype")
+        if iso and D in (64, 128) and K <= 64:
+            m = MGP_MATH_TC_ISO
+    nbytes = lib.mgp_log_density_ws_bytes(B, HW, C, K, D, m)
+    ws, cache_key = None, None
+    if m == MGP_MATH_TC_ISO and D in (64, 128) and K <= 64:
+        # the tensor-core path keeps only prototype-side operands in its workspace (plus log pi, rebuilt every call)
+        cache_key = (mu.data_ptr(), mu._version, sg.data_ptr(), sg._version, P, D, str(x.device), _stream())
+        hit = _DENSITY_OPERANDS.get(cache_key)
+        if hit is not None and hit[0].numel() >= nbytes:
+            ws, m = hit[0], MGP_MATH_TC_ISO_REUSE
+            _DENSITY_OPERANDS.move_to_end(cache_key)
+    if ws is None:
+        ws = torch.empty((max(16, nbytes),), device=x.device, dtype=torch.uint8)
+    out_c = torch.empty((B, C, HW), device=x.device, dtype=torch.float32)
+    out_a = torch.empty((B, HW), device=x.device, dtype=torch.float32) if want_all else None
+    check(lib.mgp_log_density(x.data_ptr(), mu.data_ptr(), sg.data_ptr(), w.data_ptr(), out_c.data_ptr(), _p(out_a),
+                              B, HW, C, K, D, m, ws.data_ptr(), nbytes, _stream()), "mgp_log_density")
+    if cache_key is not None and m == MGP_MATH_TC_ISO:
+        _DENSITY_OPERANDS[cache_key] = (ws, mu, sg)      # (keeps mu / sigma alive: their addresses stay theirs)
+        while len(_DENSITY_OPERANDS) > 2:
+            _DENSITY_OPERANDS.popitem(last=False)
+    _count(2 if m == MGP_MATH_TC_ISO_REUSE else 3)
+    return out_c, out_a
 
 
 @_on_device
