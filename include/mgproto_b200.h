@@ -320,6 +320,23 @@ int mgp_update_gmm(const float* bank, const void* shadow_h, const void* shadow_l
                    int32_t* adam_step, int32_t* order, int32_t* sched, float* stats, int n_split,
                    int num_em_loop, float alpha, double lr, double beta1, double beta2, double adam_eps,
                    double tau, float lamda, int C, int K, int D, int cap, void* stream);
+/* The tensor-core update_GMM of mgp_update_gmm (planner + one kernel) with STAGED outputs: mu and weight_cp are only
+ * read; the new means go to mu_stage [C,K,D] and the new class-diagonal pi to pi_stage [C,K] (pi_stage[c*K+k] is the
+ * value for weight_cp[c][c*K+k]), for every class.  exp_avg / exp_avg_sq are updated in place as in mgp_update_gmm.
+ * A caller can therefore run it on a second stream while other work still reads mu and pi, and then apply it with
+ * mgp_em_commit on the stream that owns them.  Only the tensor-core path is staged: the same preconditions (shadow,
+ * status, sigma isotropic -- asserted by calling this -- and a supported shape), else MGP_ERR_UNSUPPORTED with nothing
+ * enqueued.  The staging buffers must not alias mu / weight_cp. */
+int mgp_update_gmm_staged(const void* shadow_h, const void* shadow_l, const float* shadow_xx, int32_t* status,
+                          uint8_t* updated, const int64_t* mem_len, const float* mu, const float* sigma,
+                          const float* weight_cp, float* exp_avg, float* exp_avg_sq, int32_t* adam_step,
+                          int32_t* order, int32_t* sched, float* stats, int n_split, int num_em_loop, float alpha,
+                          double lr, double beta1, double beta2, double adam_eps, double tau, float lamda,
+                          float* mu_stage, float* pi_stage, int C, int K, int D, int cap, void* stream);
+/* mu [C,K,D] <- mu_stage, weight_cp[c][c*K+k] <- pi_stage[c*K+k]: applies mgp_update_gmm_staged's result (one launch).
+ * D % 4 == 0, mu and mu_stage 16-byte aligned. */
+int mgp_em_commit(const float* mu_stage, const float* pi_stage, float* mu, float* weight_cp, int C, int K, int D,
+                  void* stream);
 
 /* ---- a11/a13/a14  EM building blocks on explicit rows ---------------------------------------
  * ref: model.py:303-321 (_e_step), :338-365 (_m_step), :403-421 (_score).

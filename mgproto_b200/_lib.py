@@ -49,6 +49,8 @@ SIGNATURES = {
     "mgp_em_stat_stride": (_sz, [_i, _i, _i]),
     "mgp_update_gmm_launches": (_i, [_i, _i, _i, _i, _i]),
     "mgp_update_gmm": (_i, [_vp] * 4 + [_i] + [_vp] * 12 + [_i, _i] + [_f] + [_d] * 5 + [_f] + [_i] * 4 + [_vp]),
+    "mgp_update_gmm_staged": (_i, [_vp] * 15 + [_i, _i, _f] + [_d] * 5 + [_f, _vp, _vp] + [_i] * 4 + [_vp]),
+    "mgp_em_commit": (_i, [_vp] * 4 + [_i] * 3 + [_vp]),
     "mgp_em_plan": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "mgp_em_stats": (_i, [_vp, _vp, _vp, _vp, _vp, _f, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _vp]),
     "mgp_em_update": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i,

@@ -30,7 +30,8 @@ bool mgp_em_tc_supported(int K, int D, int cap);
 int mgp_em_tc_launch(const void* shadow_h, const void* shadow_l, const float* shadow_xx, const float* bias_corr, const int32_t* order,
                      const int32_t* sched, float* mu, const float* sigma, float* weight, float* exp_avg, float* exp_avg_sq,
                      int* status, int num_em_loop, float alpha, double lr, double beta1, double beta2, double adam_eps,
-                     double tau, float lamda, int C, int K, int D, int cap, cudaStream_t st);
+                     double tau, float lamda, float* mu_stage, float* pi_stage, int C, int K, int D, int cap,
+                     cudaStream_t st);
 
 namespace {
 using namespace mgp_em;
@@ -1477,6 +1478,30 @@ static int em_validate(int C, int K, int D, int cap, int num_em_loop) {
     return MGP_OK;
 }
 
+static bool em_tc_fits(const void* shadow_h, const void* shadow_l, const float* shadow_xx, const int32_t* status,
+                       int sigma_iso, int n_split, int num_em_loop, int C, int K, int D, int cap) {
+    return shadow_h && shadow_l && shadow_xx && status && em_tc_applies(K, D, cap, sigma_iso) &&
+           (size_t)5 * num_em_loop * C + 4 + C <= (size_t)C * n_split * mgp_em_stat_stride(K, D, 0);
+}
+
+#ifdef MGP_WITH_TC
+// planner + tensor-core kernel (em_tc.cu); mu_stage / pi_stage null: the new means and pi are written in place
+static int em_tc_enqueue(const void* shadow_h, const void* shadow_l, const float* shadow_xx, int32_t* status,
+                         uint8_t* updated, const int64_t* mem_len, float* mu, const float* sigma, float* weight_cp,
+                         float* exp_avg, float* exp_avg_sq, int32_t* adam_step, int32_t* order, int32_t* sched, float* stats,
+                         int num_em_loop, float alpha, double lr, double beta1, double beta2, double adam_eps, double tau,
+                         float lamda, float* mu_stage, float* pi_stage, int C, int K, int D, int cap, void* stream) {
+    // the planner also tabulates the steps' Adam bias corrections into the (otherwise unused) stats scratch
+    em_plan_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(updated, mem_len, order, sched, adam_step, 0, C, cap, num_em_loop,
+                                                         make_adam(lr, beta1, beta2, adam_eps), stats,
+                                                         reinterpret_cast<int32_t*>(stats + (size_t)5 * num_em_loop * C + 4));
+    MGP_CHECK_LAUNCH();
+    return mgp_em_tc_launch(shadow_h, shadow_l, shadow_xx, stats, order, sched, mu, sigma, weight_cp, exp_avg, exp_avg_sq,
+                            status, num_em_loop, alpha, lr, beta1, beta2, adam_eps, tau, lamda, mu_stage, pi_stage, C, K, D,
+                            cap, (cudaStream_t)stream);
+}
+#endif
+
 extern "C" int mgp_update_gmm(const float* bank, const void* shadow_h, const void* shadow_l, const float* shadow_xx,
                               int sigma_iso, int32_t* status, uint8_t* updated, const int64_t* mem_len, float* mu,
                               const float* sigma,
@@ -1490,17 +1515,10 @@ extern "C" int mgp_update_gmm(const float* bank, const void* shadow_h, const voi
     int rc = em_validate(C, K, D, cap, num_em_loop);                 // before the planner clears flags / counts steps
     if (rc != MGP_OK) return rc;
 #ifdef MGP_WITH_TC
-    if (shadow_h && shadow_l && shadow_xx && status && em_tc_applies(K, D, cap, sigma_iso) &&
-        (size_t)5 * num_em_loop * C + 4 + C <= (size_t)C * n_split * mgp_em_stat_stride(K, D, 0)) {
-        // tensor-core path: the planner also tabulates the steps' Adam bias corrections into the (otherwise unused) stats scratch
-        em_plan_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(updated, mem_len, order, sched, adam_step, 0, C, cap, num_em_loop,
-                                                             make_adam(lr, beta1, beta2, adam_eps), stats,
-                                                             reinterpret_cast<int32_t*>(stats + (size_t)5 * num_em_loop * C + 4));
-        MGP_CHECK_LAUNCH();
-        return mgp_em_tc_launch(shadow_h, shadow_l, shadow_xx, stats, order, sched, mu, sigma, weight_cp, exp_avg, exp_avg_sq,
-                                status, num_em_loop, alpha, lr, beta1, beta2, adam_eps, tau, lamda, C, K, D, cap,
-                                (cudaStream_t)stream);
-    }
+    if (em_tc_fits(shadow_h, shadow_l, shadow_xx, status, sigma_iso, n_split, num_em_loop, C, K, D, cap))
+        return em_tc_enqueue(shadow_h, shadow_l, shadow_xx, status, updated, mem_len, mu, sigma, weight_cp, exp_avg,
+                             exp_avg_sq, adam_step, order, sched, stats, num_em_loop, alpha, lr, beta1, beta2, adam_eps,
+                             tau, lamda, nullptr, nullptr, C, K, D, cap, stream);
 #endif
     rc = mgp_em_plan(updated, mem_len, order, sched, adam_step, 0, C, cap, num_em_loop, stream);
     if (rc != MGP_OK) return rc;
@@ -1542,6 +1560,57 @@ extern "C" int mgp_update_gmm(const float* bank, const void* shadow_h, const voi
     }
     return mgp_em_update(nullptr, n_split, 0, cap, order, sched, mu, sigma, weight_cp, exp_avg, exp_avg_sq, 0,
                          num_em_loop, 2, lr, beta1, beta2, adam_eps, tau, lamda, nullptr, -1, C, K, D, stream);
+}
+
+extern "C" int mgp_update_gmm_staged(const void* shadow_h, const void* shadow_l, const float* shadow_xx, int32_t* status,
+                                     uint8_t* updated, const int64_t* mem_len, const float* mu, const float* sigma,
+                                     const float* weight_cp, float* exp_avg, float* exp_avg_sq, int32_t* adam_step,
+                                     int32_t* order, int32_t* sched, float* stats, int n_split, int num_em_loop, float alpha,
+                                     double lr, double beta1, double beta2, double adam_eps, double tau, float lamda,
+                                     float* mu_stage, float* pi_stage, int C, int K, int D, int cap, void* stream) {
+    if (!shadow_h || !shadow_l || !shadow_xx || !status || !updated || !mem_len || !mu || !sigma || !weight_cp ||
+        !exp_avg || !exp_avg_sq || !adam_step || !order || !sched || !stats || !mu_stage || !pi_stage || n_split <= 0)
+        return MGP_ERR_INVALID;
+    const int rc = em_validate(C, K, D, cap, num_em_loop);
+    if (rc != MGP_OK) return rc;
+    if (mu_stage == mu || (const float*)pi_stage == weight_cp) return MGP_ERR_INVALID;
+#ifdef MGP_WITH_TC
+    if (em_tc_fits(shadow_h, shadow_l, shadow_xx, status, 1, n_split, num_em_loop, C, K, D, cap))
+        // the kernel only reads mu and weight_cp (the staged outputs take the writes)
+        return em_tc_enqueue(shadow_h, shadow_l, shadow_xx, status, updated, mem_len, const_cast<float*>(mu), sigma,
+                             const_cast<float*>(weight_cp), exp_avg, exp_avg_sq, adam_step, order, sched, stats,
+                             num_em_loop, alpha, lr, beta1, beta2, adam_eps, tau, lamda, mu_stage, pi_stage, C, K, D, cap,
+                             stream);
+#endif
+    return MGP_ERR_UNSUPPORTED;                                      // nothing enqueued: no flag cleared, no step counted
+}
+
+namespace {
+// mu <- mu_stage (float4), and pi_stage [C,K] into weight_cp's class-diagonal blocks
+__global__ void __launch_bounds__(256)
+em_commit_kernel(const float4* __restrict__ mu_stage, const float* __restrict__ pi_stage, float4* __restrict__ mu,
+                 float* __restrict__ weight_cp, int n4, int C, int K) {
+    const int stride = gridDim.x * blockDim.x;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) mu[i] = mu_stage[i];
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < C * K; i += stride) {
+        const int c = i / K;
+        weight_cp[(size_t)c * C * K + i] = pi_stage[i];             // row c, column c K + k
+    }
+}
+}  // namespace
+
+extern "C" int mgp_em_commit(const float* mu_stage, const float* pi_stage, float* mu, float* weight_cp, int C, int K, int D,
+                             void* stream) {
+    if (!mu_stage || !pi_stage || !mu || !weight_cp || C <= 0 || K <= 0 || D <= 0 || (D & 3)) return MGP_ERR_INVALID;
+    if (!mgp_aligned16(mu_stage) || !mgp_aligned16(mu)) return MGP_ERR_INVALID;
+    if ((long long)C * K * D > 0x7fffffffLL) return MGP_ERR_UNSUPPORTED;
+    const int n4 = C * K * D / 4;
+    int blocks = (n4 + 255) / 256;
+    if (blocks > 1024) blocks = 1024;
+    em_commit_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const float4*>(mu_stage), pi_stage,
+                                                               reinterpret_cast<float4*>(mu), weight_cp, n4, C, K);
+    MGP_CHECK_LAUNCH();
+    return MGP_OK;
 }
 
 extern "C" int mgp_em_estep(const float* x, const float* mu, const float* sigma, const float* pi, float* log_resp,

@@ -32,6 +32,9 @@
 // block indices, so while they fit one CTA per SM none shares its SM with another active class.  At D = 256 (one CTA
 // per SM in any case) block b runs class b.
 // HBM/L2 traffic: num_em_loop x (4 D + 4) bytes per bank row -- the algorithmic bytes of SURVEY 8(d) K-D.
+// Staged outputs (mgp_update_gmm_staged): the new means go to a [C,K,D] copy and the new class-diagonal pi to a [C,K]
+// copy instead of the parameters, so that a backward still reading mu and pi can run beside the kernel; every class
+// (inactive and skipped ones included) writes its slots, and mgp_em_commit copies them over afterwards.
 #include <cuda.h>
 #include <cuda_fp16.h>
 
@@ -64,6 +67,8 @@ struct EmTcParams {
     float* weight;
     float* exp_avg;
     float* exp_avg_sq;
+    float* mu_out;                // where the new means go: mu itself, or a staging [C,K,D] copy (see mgp_update_gmm_staged)
+    float* pi_out;                // staging [C,K] for the new class-diagonal pi, or nullptr: written into weight in place
     int* status;                  // set to 1 if a class turned out to have anisotropic sigma (its update is skipped)
     long long* prof;              // profiling (mgp_debug_set_ptr("em_tc_prof")): clock64 stamps of class `prof_class`
     AdamCfg adam;
@@ -255,7 +260,7 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
         for (int k = 0; k < KT; ++k)
             if (k < K) {
                 const size_t o = (size_t)c * KD + k * D + tid;
-                prm.mu[o] = p_[k]; prm.exp_avg[o] = m_[k]; prm.exp_avg_sq[o] = v_[k];
+                prm.mu_out[o] = p_[k]; prm.exp_avg[o] = m_[k]; prm.exp_avg_sq[o] = v_[k];
             }
     };
 
@@ -264,6 +269,7 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
         __syncthreads();
         replay(step0, L * n_active, s_misc);
         write_back();
+        if (prm.pi_out && tid < K) prm.pi_out[(size_t)c * K + tid] = prm.weight[(size_t)c * P + (size_t)c * K + tid];
         return;
     }
     // the two replays' block-wide sums depend on the plan only: two otherwise idle warps evaluate them under the set-up
@@ -299,6 +305,14 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
     const bool iso = __syncthreads_and(same ? 1 : 0) != 0;
     if (!iso) {                                      // the host promised isotropic sigma: flag it, leave the class untouched
         if (tid == 0) atomicExch(prm.status, 1);
+        if (prm.pi_out) {                            // staged: the class's staging slots keep its current values
+            if (own) {
+#pragma unroll
+                for (int k = 0; k < KT; ++k)
+                    if (k < K) prm.mu_out[(size_t)c * KD + k * D + tid] = p_[k];
+            }
+            if (tid < K) prm.pi_out[(size_t)c * K + tid] = s_pi[tid];
+        }
         return;
     }
     if (tid == 0) MGP_PROF(63, 2);
@@ -659,7 +673,10 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
     replay(step0 + L * (ord + 1), L * (n_active - ord - 1), s_misc + 4);
     if (tid == 0) MGP_PROF(63, 5);
     write_back();
-    if (tid < K) prm.weight[(size_t)c * P + (size_t)c * K + tid] = s_pi[tid];
+    if (tid < K) {
+        if (prm.pi_out) prm.pi_out[(size_t)c * K + tid] = s_pi[tid];
+        else prm.weight[(size_t)c * P + (size_t)c * K + tid] = s_pi[tid];
+    }
     if (tid == 0) MGP_PROF(63, 6);
 }
 
@@ -684,7 +701,8 @@ bool mgp_em_tc_supported(int K, int D, int cap) {
 int mgp_em_tc_launch(const void* shadow_h, const void* shadow_l, const float* shadow_xx, const float* bias_corr, const int32_t* order,
                      const int32_t* sched, float* mu, const float* sigma, float* weight, float* exp_avg, float* exp_avg_sq,
                      int* status, int num_em_loop, float alpha, double lr, double beta1, double beta2, double adam_eps,
-                     double tau, float lamda, int C, int K, int D, int cap, cudaStream_t st) {
+                     double tau, float lamda, float* mu_stage, float* pi_stage, int C, int K, int D, int cap,
+                     cudaStream_t st) {
     CUtensorMap mh, ml;                             // boxes of em_rows(D) rows: one tile, hi and lo
     const uint64_t rows = (uint64_t)C * cap;
     if (!make_map_f16(&mh, shadow_h, rows, D, em_rows(D)) || !make_map_f16(&ml, shadow_l, rows, D, em_rows(D)))
@@ -692,6 +710,7 @@ int mgp_em_tc_launch(const void* shadow_h, const void* shadow_l, const float* sh
     EmTcParams prm;
     prm.xx = shadow_xx; prm.bc = bias_corr; prm.order = order; prm.sched = sched; prm.mu = mu; prm.sigma = sigma; prm.weight = weight;
     prm.exp_avg = exp_avg; prm.exp_avg_sq = exp_avg_sq; prm.status = status;
+    prm.mu_out = mu_stage ? mu_stage : mu; prm.pi_out = pi_stage;
     prm.adam = make_adam(lr, beta1, beta2, adam_eps);
     prm.alpha = alpha; prm.tau = (float)tau; prm.omtau = (float)(1.0 - tau); prm.lamda = lamda;
     prm.num_em_loop = num_em_loop; prm.C = C; prm.K = K; prm.cap = cap;

@@ -119,6 +119,13 @@ class MGProto(nn.Module):
         self.overlap_enqueue = False     # multi-GPU: True = all-gather + enqueue on a side stream behind the backward (the
                                          # NCCL kernel and the backward kernels delay each other), False = inline on the main stream
         self._side_stream = None
+        self.overlap_em = True           # single replica, tensor-core EM: update_GMM runs the EM on a high-priority side
+                                         # stream that starts where head() enqueued the bank rows, beside the loss and
+                                         # the backward; the EM writes staged copies of mu / pi (the backward still reads
+                                         # them), committed on the caller's stream.  False = in place on the caller's stream
+        self._em_stream = None
+        self._em_fork = None             # (event, stream, capturing, versions) that head() recorded after the enqueue
+        self._em_bufs = None             # (key, persistent planner scratch + staging of the overlapped EM)
         self._em_status = None           # int32[1] on the device: set by the tensor-core EM kernel if sigma was not isotropic
         self._adam_step_dev = None       # int32[1] on the device: Adam step count, advanced by update_GMM's planner
         self._adam_step_seen = None      # host value the device counter was seeded from / last folded back to
@@ -185,6 +192,8 @@ class MGProto(nn.Module):
                     top1, rows = ops.mined_gather(xhat, idx, gt, HWn, self.num_classes, Kn)
                     ops.bank_enqueue(q.bank, q.mem_len, q.head, q.updated, rows, top1, gt, shadow=q.shadow_if_valid())
                 self.iteration_counter += 1                                       # ref :252
+                if self.em_group is None and self.overlap_em:
+                    self._mark_em_fork()
         return logits
 
     @torch.no_grad()
@@ -321,6 +330,7 @@ class MGProto(nn.Module):
         sufficient statistics are all-reduced once per EM loop (parallel.py)."""
         q = self.queue
         self.wait_enqueue()
+        fork, self._em_fork = self._em_fork, None
         C, K, D = self.prototype_means.shape
         cap = q.cap_cls
         dev = self.prototype_means.device
@@ -346,8 +356,10 @@ class MGProto(nn.Module):
         st = self._adam_state()
         self._hook_optimizer()
         host_step = int(st["step"])
+        fresh = False                    # set-up work was just enqueued on the caller's stream: the EM must follow it
         if self._adam_step_dev is None or self._adam_step_dev.device != dev or self._adam_step_seen is None or \
                 host_step != self._adam_step_seen:
+            fresh = True
             # first call, or the optimiser state was replaced / stepped elsewhere: (re)seed the device counter
             if self._em_dirty and self._adam_step_dev is not None and self._adam_step_seen is not None:
                 host_step += int(self._adam_step_dev.item()) - self._adam_step_seen   # keep the steps not folded back yet
@@ -361,9 +373,16 @@ class MGProto(nn.Module):
             # (one cached host check: prototype_covs never changes in the reference's loop) -- needs the bank's shadow
             shadow, iso = None, False
             if 2 <= K <= 16 and D in (128, 256) and ops.sigma_is_isotropic(self.prototype_covs):
+                fresh = fresh or q.shadow_if_valid() is None
                 shadow, iso = q.ensure_shadow(), True
                 if self._em_status is None or self._em_status.device != dev:
                     self._em_status = torch.zeros(1, dtype=torch.int32, device=dev)
+                    fresh = True
+            if iso and not fresh and self._em_fork_holds(fork) and \
+                    self._update_GMM_overlapped(fork[0], shadow, st, n_split, L, lr, b1, b2, eps):
+                self._em_dirty = True
+                self._bump_versions()
+                return
             ops.update_gmm(q.bank, q.updated, q.mem_len, mu, sg, wt, st["exp_avg"], st["exp_avg_sq"], self._adam_step_dev,
                            order, sched, stats, n_split, L, self.alpha, lr, b1, b2, eps, self.tau, shadow=shadow,
                            sigma_iso=iso, status=self._em_status)
@@ -387,6 +406,72 @@ class MGProto(nn.Module):
                       lr, b1, b2, eps, self.tau)
         self._em_dirty = True
         self._bump_versions()
+
+    def _em_versions(self):
+        """Identity and version counter of everything the EM reads or writes besides its own scratch."""
+        opt = self.prototype_optimizer
+        st = opt.state.get(self.prototype_means, {}) if opt is not None else {}
+        b = self.queue._buffers
+        ts = (self.prototype_means, self.prototype_covs, self.last_layer.weight, st.get("exp_avg"), st.get("exp_avg_sq"),
+              b["bank"], b["updated"], b["mem_len"], b["head"])
+        return tuple(None if t is None else (id(t), t._version) for t in ts)
+
+    def _mark_em_fork(self):
+        """head(): the bank rows of this step are enqueued -- the point from which update_GMM's EM may run."""
+        cur = torch.cuda.current_stream(self.prototype_means.device)
+        ev = torch.cuda.Event()
+        ev.record(cur)
+        self._em_fork = (ev, cur, torch.cuda.is_current_stream_capturing(), self._em_versions())
+
+    def _em_fork_holds(self, fork):
+        """The EM may start at head()'s fork: same stream and capture state, and nothing it reads or writes (the
+        parameters, the Adam moments, the bank and its flags) changed in between -- else it runs after everything the
+        caller's stream has enqueued, as it always did.  (A write through ``.data`` is invisible to the version counter.)"""
+        if fork is None or not self.overlap_em:
+            return False
+        _, stream, capturing, versions = fork
+        return (stream == torch.cuda.current_stream(self.prototype_means.device)
+                and capturing == torch.cuda.is_current_stream_capturing() and versions == self._em_versions())
+
+    def _update_GMM_overlapped(self, fork_event, shadow, st, n_split, L, lr, b1, b2, eps):
+        """The tensor-core EM on the side stream from ``fork_event`` on, with staged outputs: the loss and backward the
+        caller enqueued after head() still read mu (proto_weight_kernel) and pi (head_bwd_kernel) and run beside it on
+        the SMs it leaves idle.  The caller's stream then waits for the EM and commits mu / pi, so that stream order
+        after this call is what the in-place path leaves.  False (nothing enqueued) if the persistent buffers would
+        have to be allocated during a graph capture, or if the tensor-core kernel does not take the call."""
+        q = self.queue
+        C, K, D = self.prototype_means.shape
+        dev = self.prototype_means.device
+        cur = torch.cuda.current_stream(dev)
+        if self._em_stream is None or self._em_stream.device != dev:
+            # highest priority (out-of-range values map to the device's greatest): the EM's CTAs are dispatched ahead
+            # of the backward's, which would otherwise take the register file of the SMs the EM needs
+            self._em_stream = torch.cuda.Stream(device=dev, priority=-100)
+        side = self._em_stream
+        key = (dev, C, K, D, n_split)
+        if self._em_bufs is None or self._em_bufs[0] != key:
+            if torch.cuda.is_current_stream_capturing():
+                return False
+            # persistent, and allocated on the side stream: no block the caller's stream frees can be handed out here
+            with torch.cuda.stream(side):
+                f32, i32 = torch.float32, torch.int32
+                self._em_bufs = (key, (torch.empty(C, dtype=i32, device=dev), torch.empty(2, dtype=i32, device=dev),
+                                       torch.empty((C, n_split, ops.em_stat_stride(K, D)), dtype=f32, device=dev),
+                                       torch.empty((C, K, D), dtype=f32, device=dev),
+                                       torch.empty((C, K), dtype=f32, device=dev)))
+        order, sched, stats, mu_stage, pi_stage = self._em_bufs[1]
+        mu, sg, wt = self.prototype_means.data, self.prototype_covs.data, self.last_layer.weight.data
+        side.wait_event(fork_event)
+        with torch.cuda.stream(side):
+            if not ops.update_gmm_staged(q.updated, q.mem_len, mu, sg, wt, st["exp_avg"], st["exp_avg_sq"],
+                                         self._adam_step_dev, order, sched, stats, n_split, L, self.alpha, lr, b1, b2, eps,
+                                         self.tau, mu_stage, pi_stage, shadow, self._em_status):
+                return False
+            join = torch.cuda.Event()
+            join.record(side)
+        cur.wait_event(join)
+        ops.em_commit(mu_stage, pi_stage, mu, wt)
+        return True
 
     def _bump_versions(self):
         """The EM kernels write the means and the mixture weights through raw pointers: tell torch (autograd's

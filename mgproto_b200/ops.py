@@ -654,6 +654,38 @@ def update_gmm(bank, updated, mem_len, mu_ckd, sigma_ckd, weight_cp, exp_avg, ex
 
 
 @_on_device
+def update_gmm_staged(updated, mem_len, mu_ckd, sigma_ckd, weight_cp, exp_avg, exp_avg_sq, adam_step, order, sched, stats,
+                      n_split, num_em_loop, alpha, lr, beta1, beta2, adam_eps, tau, mu_stage, pi_stage, shadow, status,
+                      lamda=1.0):
+    """The tensor-core update_gmm with its new means / class-diagonal pi written to ``mu_stage`` [C,K,D] and
+    ``pi_stage`` [C,K] instead of ``mu_ckd`` / ``weight_cp`` (which it only reads); ``em_commit`` applies them.
+    -> False, with nothing enqueued, if the tensor-core kernel does not take this call (shape, or the em_tc option)."""
+    C, K, D = mu_ckd.shape
+    cap = shadow[2].shape[1]
+    rc = _lib.load().mgp_update_gmm_staged(_p(shadow[0]), _p(shadow[1]), _p(shadow[2]), _p(status), updated.data_ptr(),
+                                            mem_len.data_ptr(), mu_ckd.data_ptr(), sigma_ckd.data_ptr(),
+                                            weight_cp.data_ptr(), exp_avg.data_ptr(), exp_avg_sq.data_ptr(),
+                                            adam_step.data_ptr(), order.data_ptr(), sched.data_ptr(), stats.data_ptr(),
+                                            int(n_split), int(num_em_loop), float(alpha), float(lr), float(beta1),
+                                            float(beta2), float(adam_eps), float(tau), float(lamda), mu_stage.data_ptr(),
+                                            pi_stage.data_ptr(), C, K, D, cap, _stream())
+    if rc == -2:                                                              # MGP_ERR_UNSUPPORTED
+        return False
+    check(rc, "mgp_update_gmm_staged")
+    _count(2)
+    return True
+
+
+@_on_device
+def em_commit(mu_stage, pi_stage, mu_ckd, weight_cp):
+    """mu_ckd <- mu_stage, weight_cp's class-diagonal blocks <- pi_stage [C,K] (one launch)."""
+    C, K, D = mu_ckd.shape
+    check(_lib.load().mgp_em_commit(mu_stage.data_ptr(), pi_stage.data_ptr(), mu_ckd.data_ptr(), weight_cp.data_ptr(),
+                                    C, K, D, _stream()), "mgp_em_commit")
+    _count(1)
+
+
+@_on_device
 def em_estep(x_nd, mu_kd, sigma_kd, pi_k, want_log_resp=True, want_score=True):
     """ref model.py:303-321 / :403-421 -> (log_resp [n,K] | None, score [n] | None)."""
     x = _req(x_nd.contiguous(), torch.float32, "x")
