@@ -374,6 +374,40 @@ int mgp_push_argmin(const float* logp_bphw, const int64_t* labels, int32_t* arg,
 int mgp_push_argmin_top1(const unsigned long long* best_bp, const int64_t* labels, int32_t* arg,
                          float* val, int B, int C, int K, void* stream);
 
+/* ---- f1  prototype projection: candidate store and greedy assignment ----------------------------
+ * ref: push.py:125-200.  Prototype (c,k) picks among images labelled c, after prototypes 0..k-1 of its class, so its
+ * pick is among its own k+1 best candidates: a store of the K best candidates per prototype (K <= 64) gives the
+ * reference's greedy exactly, in C*K*K*(D+4)*4 bytes whatever the number of images.  Candidates are ordered by
+ * (-p ascending, image id ascending); exact ties in -p go to the smaller id.  The store is the set of the K smallest
+ * keys merged so far, independent of the order of the merges: image-sharded replicas that merge the same gathered
+ * records end with identical stores.
+ *
+ * Records: one per image, rec_stride fp32 words apart (a multiple of 4, >= K*D + 2K + 2); rec_rows / rec_val /
+ * rec_patch / rec_label point at the fields of record 0: rows [K*D] fp32 (16-byte aligned), val [K] fp32 (-p),
+ * patch [K] int32, label int64 (8-byte aligned).  A record whose label is outside [0, C) is ignored; a candidate whose
+ * patch is < 0 is ignored.
+ *
+ * mgp_push_records (ref push.py:125-158): per image b, from mgp_push_argmin(_top1)'s arg [B,K] / val [B,K] and the
+ * normalised features xhat_nd [B*HW, D], the rows xhat_nd[b*HW + arg[b,k]], the values, the patches and the label
+ * (written as -1 outside [0, C); then nothing is read from arg / val / xhat_nd for that image).
+ *
+ * mgp_push_merge: folds n records into the store, record i being image id0 + i (id0 + n <= 0xffffffff).  Store:
+ * key [C,K,K] uint64 = (monotone key of -p) << 32 | id, empty slot = UINT64_MAX (fill it so before the first merge);
+ * patch [C,K,K] int32; row [C,K,K,D] fp32 (16-byte aligned).  One image id must not be merged twice.
+ *
+ * mgp_push_assign (ref push.py:165-200): per class, k = 0..K-1 in order, the smallest key of prototype (c,k) whose id
+ * no earlier prototype of the class took: its row is copied into mu [C,K,D] (16-byte aligned), chosen_id /
+ * chosen_patch [C*K] int64 and chosen_val [C*K] fp32 (-p) receive the pick.  Without a candidate: id -1, patch -1,
+ * val +inf, mu[c,k] untouched. */
+int mgp_push_records(const int32_t* arg, const float* val, const float* xhat_nd, const int64_t* labels,
+                     float* rec_rows, float* rec_val, int32_t* rec_patch, int64_t* rec_label, int rec_stride,
+                     int B, int HW, int C, int K, int D, void* stream);
+int mgp_push_merge(const float* rec_rows, const float* rec_val, const int32_t* rec_patch, const int64_t* rec_label,
+                   int rec_stride, int n, size_t id0, unsigned long long* key, int32_t* patch, float* row,
+                   int C, int K, int D, void* stream);
+int mgp_push_assign(const unsigned long long* key, const int32_t* patch, const float* row, float* mu,
+                    int64_t* chosen_id, int64_t* chosen_patch, float* chosen_val, int C, int K, int D, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -63,6 +63,9 @@ SIGNATURES = {
     "mgp_mine_ce": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _f, _vp]),
     "mgp_push_argmin": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "mgp_push_argmin_top1": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "mgp_push_records": (_i, [_vp] * 8 + [_i] * 6 + [_vp]),
+    "mgp_push_merge": (_i, [_vp] * 4 + [_i, _i, _sz] + [_vp] * 3 + [_i] * 3 + [_vp]),
+    "mgp_push_assign": (_i, [_vp] * 7 + [_i] * 3 + [_vp]),
 }
 
 _lib = None

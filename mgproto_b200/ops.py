@@ -19,7 +19,7 @@ from ._lib import (MGP_MATH_AUTO, MGP_MATH_FP32, MGP_MATH_TC, MGP_MATH_TC_ISO, M
                    check)
 
 __all__ = ["normalize_fwd", "logprob", "log_density", "logprob_top1", "head_select", "head_select_top1", "head_level0", "head_forward", "HeadFunction", "mined_gather", "bank_enqueue",
-           "bank_linearize", "bank_shadow_sync", "em_plan", "em_stats", "em_update", "update_gmm", "em_estep", "em_mstep_closed", "em_mstep_div", "topt_pool", "ood_score", "push_argmin", "push_argmin_top1", "mine_cross_entropy",
+           "bank_linearize", "bank_shadow_sync", "em_plan", "em_stats", "em_update", "update_gmm", "em_estep", "em_mstep_closed", "em_mstep_div", "topt_pool", "ood_score", "push_argmin", "push_argmin_top1", "push_records", "push_store", "push_merge", "push_assign", "mine_cross_entropy",
            "MATH_MODES"]
 
 MATH_MODES = {"fp32": MGP_MATH_FP32, "tc": MGP_MATH_TC, "auto": MGP_MATH_AUTO, "tc_reuse": MGP_MATH_TC_REUSE,
@@ -839,3 +839,88 @@ def push_argmin(logp_bphw, labels, C, K):
                                       _stream()), "mgp_push_argmin")
     _count(1)
     return arg, val
+
+
+def _push_rec_stride(K, D):
+    """fp32 words of one packed push record: the mined record layout (_rec_stride) with K more fp32 words in its row
+    block, which hold the K values -p."""
+    return _rec_stride(K, D + 1)
+
+
+def _push_rec_views(rec, K, D):
+    """(rows [b, K*D] fp32, val [b, K] fp32 (-p), patch [b, K] int32, label [b] int64) views into push records
+    [b, _push_rec_stride(K, D)]: the fields of _rec_views(rec, K, D + 1), whose row block is split into rows and val."""
+    ext, patch, label = _rec_views(rec, K, D + 1)
+    return ext[:, :K * D], ext[:, K * D:], patch, label
+
+
+def push_padding_records(n, K, D, device):
+    """n push records that every merge ignores (label -1): what a rank contributes for images it does not have."""
+    rec = torch.empty((n, _push_rec_stride(K, D)), device=device, dtype=torch.float32)
+    _push_rec_views(rec, K, D)[3].fill_(-1)
+    return rec
+
+
+@_on_device
+def push_records(arg, val, xhat_nd, labels, C, HW, n_out=None):
+    """ref push.py:125-158: per image, the K candidate rows xhat_nd[b*HW + arg[b,k]], the values val [B,K], the patches
+    and the label, packed into one record per image (_push_rec_views) -- the unit a sharded push all-gathers.
+    n_out >= B: records B..n_out-1 are padding (label -1)."""
+    _req(arg, torch.int32, "arg")
+    _req(val, torch.float32, "val")
+    _req(xhat_nd, torch.float32, "xhat")
+    lab = _req(labels, torch.int64, "labels")
+    B, K = arg.shape
+    D = xhat_nd.shape[1]
+    n_out = B if n_out is None else int(n_out)
+    if n_out < B or val.shape != (B, K) or lab.shape != (B,) or xhat_nd.shape[0] != B * HW:
+        raise RuntimeError("mgproto_b200: push_records shape mismatch")
+    rec = push_padding_records(n_out, K, D, arg.device)
+    rows, v, patch, label = _push_rec_views(rec, K, D)
+    check(_lib.load().mgp_push_records(arg.data_ptr(), val.data_ptr(), xhat_nd.data_ptr(), lab.data_ptr(),
+                                       rows.data_ptr(), v.data_ptr(), patch.data_ptr(), label.data_ptr(),
+                                       rec.shape[1], B, HW, C, K, D, _stream()), "mgp_push_records")
+    _count(1)
+    return rec
+
+
+def push_store(C, K, D, device):
+    """Empty candidate store of a push: (key [C,K,K] int64 holding the uint64 keys, all bits set = empty slot;
+    patch [C,K,K] int32; row [C,K,K,D] fp32) -- C*K*K*(D+4)*4 bytes, whatever the size of the push set."""
+    return (torch.full((C, K, K), -1, device=device, dtype=torch.int64),
+            torch.empty((C, K, K), device=device, dtype=torch.int32),
+            torch.empty((C, K, K, D), device=device, dtype=torch.float32))
+
+
+@_on_device
+def push_merge(rec, store, id0):
+    """Fold push records [n, stride] into ``store`` (push_store) in place; record i is image id0 + i.  The store keeps,
+    per prototype, the K smallest (-p, image id) over everything merged, whatever the order of the merges."""
+    key, patch, row = store
+    C, K, _, D = row.shape
+    rec = _req(rec, torch.float32, "records")
+    if rec.dim() != 2 or rec.shape[1] != _push_rec_stride(K, D):
+        raise RuntimeError("mgproto_b200: push_merge records must be [n, %d]" % _push_rec_stride(K, D))
+    rows, v, pt, label = _push_rec_views(rec, K, D)
+    check(_lib.load().mgp_push_merge(rows.data_ptr(), v.data_ptr(), pt.data_ptr(), label.data_ptr(), rec.shape[1],
+                                     rec.shape[0], int(id0), key.data_ptr(), patch.data_ptr(), row.data_ptr(), C, K, D,
+                                     _stream()), "mgp_push_merge")
+    _count(1)
+
+
+@_on_device
+def push_assign(store, mu_ckd):
+    """ref push.py:165-200 from the store: the greedy per class, each pick's row written into mu_ckd [C,K,D] in place
+    through its raw pointer (the caller advances its version).  -> int64 [3, C*K] on the device: row 0 the image id,
+    row 1 the patch (-1 both where no image was left), row 2 the -p of the pick as float32 in its first C*K float32
+    words (+inf where none): one buffer, so one copy brings the whole result to the host."""
+    key, patch, row = store
+    C, K, _, D = row.shape
+    mu = _req(mu_ckd, torch.float32, "mu")
+    if mu.shape != (C, K, D):
+        raise RuntimeError("mgproto_b200: push_assign mu must be [%d, %d, %d]" % (C, K, D))
+    out = torch.empty((3, C * K), device=mu.device, dtype=torch.int64)
+    check(_lib.load().mgp_push_assign(key.data_ptr(), patch.data_ptr(), row.data_ptr(), mu.data_ptr(), out[0].data_ptr(),
+                                      out[1].data_ptr(), out[2].data_ptr(), C, K, D, _stream()), "mgp_push_assign")
+    _count(1)
+    return out
