@@ -362,6 +362,25 @@ int mgp_em_mstep_div(const float* x, const float* log_resp, const float* mu, con
 int mgp_mine_ce(const float* out, const int64_t* gt, float* loss_b, float* grad, int B, int C, int T,
                 float mine_coef, void* stream);
 
+/* ---- a17b  auxiliary loss on the embedding: the Proxy-Anchor criterion ---------------------------
+ * ref: utils/losses.py:19-61 (l2_norm, Proxy_Anchor.forward), called at train_and_test.py:42; it replaces the host
+ * one-hot encoding (:9-16), the host read of the number of positive proxies (:51-52) and autograd's backward.
+ * x [B,E] embeddings of element type x_dtype (MGP_X_F32 / _BF16 / _F16, no layout flag), proxies [C,E] fp32,
+ * labels [B] int64.  With xh_b = x_b / sqrt(|x_b|^2 + 1e-12), ph_c likewise and s_bc = xh_b . ph_c:
+ *   loss [1] = (1/|C+|) sum_c log(1 + sum_{b: t_b = c} exp(-beta (s_bc - margin)))
+ *            + (1/C)    sum_c log(1 + sum_{b: t_b != c} exp(beta (s_bc + margin))),   C+ = classes present in the batch;
+ *   grad_x [B,E] = d loss / d x in x's element type (round to nearest even), grad_p [C,E] = d loss / d proxies, fp32,
+ *   both through the normalisations; either may be NULL (then that pass is skipped);
+ *   n_valid (int32 [1], may be NULL) = |C+|.
+ * Beyond the reference: an image whose label is outside [0, C) contributes to no sum (and gets a zero gradient);
+ * |C+| = 0 gives the second term alone; C = 2 is allowed.  One launch of one cluster, no atomics (bit-identical from
+ * run to run), nothing read back by the host, safe under stream capture.
+ * 1 <= B <= 4096, 2 <= C <= 4096, E % 4 == 0, E <= 512 (MGP_ERR_UNSUPPORTED otherwise); x, proxies, grad_x and
+ * grad_p 16-byte aligned. */
+int mgp_proxy_anchor(const void* x, int x_dtype, const float* proxies, const int64_t* labels, int B, int C, int E,
+                     float margin, float beta, float* loss, void* grad_x, float* grad_p, int32_t* n_valid,
+                     void* stream);
+
 /* ---- f1  prototype projection search --------------------------------------------------------
  * ref: push.py:125-158.  For every image and the K prototypes of its label's class: flat HW
  * argmin of -p (= argmax of log p; ties: smaller index) and -p there.

@@ -9,11 +9,11 @@ from . import _lib
 
 _lib.load()   # fail loudly at import if the CUDA library is missing -- there is no fallback
 
-from . import ops  # noqa: E402
+from . import losses, ops  # noqa: E402
 from .memory import MemoryBank  # noqa: E402
 from .model import (MGProto, NonNegLinear, construct_MGProto, l2_normalize, momentum_update)  # noqa: E402
 from .push import push_prototypes  # noqa: E402
 
 __all__ = ["MGProto", "NonNegLinear", "MemoryBank", "construct_MGProto", "l2_normalize", "momentum_update", "ops",
-           "push_prototypes"]
+           "push_prototypes", "losses"]
 __version__ = "0.1.0"

@@ -61,6 +61,7 @@ SIGNATURES = {
     "mgp_ood_score": (_i, [_vp, _i, _i, _vp, _vp, _vp, _i, _i, _vp]),
     "mgp_topt_pool": (_i, [_vp] * 5 + [_i] * 6 + [_vp]),
     "mgp_mine_ce": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _f, _vp]),
+    "mgp_proxy_anchor": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _f, _f, _vp, _vp, _vp, _vp, _vp]),
     "mgp_push_argmin": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "mgp_push_argmin_top1": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "mgp_push_records": (_i, [_vp] * 8 + [_i] * 6 + [_vp]),

@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libmgproto_b200.so")
 STAMP = LIB + ".stamp"
-SOURCES = ["abi.cu", "normalize.cu", "logprob_simt.cu", "logprob_tc.cu", "logprob_tcz.cu", "log_density.cu", "head.cu", "bank.cu", "em.cu", "em_tc.cu", "em_api.cu", "push.cu"]
+SOURCES = ["abi.cu", "normalize.cu", "logprob_simt.cu", "logprob_tc.cu", "logprob_tcz.cu", "log_density.cu", "head.cu", "bank.cu", "em.cu", "em_tc.cu", "em_api.cu", "push.cu", "aux_loss.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--use_fast_math=false",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v", "-DMGP_WITH_TC"]
 

@@ -20,6 +20,7 @@ from ._lib import (MGP_MATH_AUTO, MGP_MATH_FP32, MGP_MATH_TC, MGP_MATH_TC_ISO, M
 
 __all__ = ["normalize_fwd", "logprob", "log_density", "logprob_top1", "head_select", "head_select_top1", "head_level0", "head_forward", "HeadFunction", "mined_gather", "bank_enqueue",
            "bank_linearize", "bank_shadow_sync", "em_plan", "em_stats", "em_update", "update_gmm", "em_estep", "em_mstep_closed", "em_mstep_div", "topt_pool", "ood_score", "push_argmin", "push_argmin_top1", "push_records", "push_store", "push_merge", "push_assign", "mine_cross_entropy",
+           "proxy_anchor", "ProxyAnchorFunction",
            "MATH_MODES"]
 
 MATH_MODES = {"fp32": MGP_MATH_FP32, "tc": MGP_MATH_TC, "auto": MGP_MATH_AUTO, "tc_reuse": MGP_MATH_TC_REUSE,
@@ -924,3 +925,56 @@ def push_assign(store, mu_ckd):
                                       out[1].data_ptr(), out[2].data_ptr(), C, K, D, _stream()), "mgp_push_assign")
     _count(1)
     return out
+
+
+# ----------------------------------------------------------------------------------- a17b (auxiliary loss)
+@_on_device
+def _proxy_anchor(x, proxies, labels, margin, beta, want_gx, want_gp):
+    """One launch of mgp_proxy_anchor -> (loss [1], grad_x or None, grad_p or None, n_valid int32 [1])."""
+    code = _FEATURE_DTYPES.get(x.dtype) if isinstance(x, torch.Tensor) else None
+    if code is None:
+        raise RuntimeError("mgproto_b200: embeddings must be a torch.float32, torch.bfloat16 or torch.float16 tensor")
+    x = _req(x.contiguous(), x.dtype, "embeddings")
+    p = _req(proxies.contiguous(), torch.float32, "proxies")
+    t = _req(labels.contiguous(), torch.int64, "labels")
+    if x.dim() != 2 or p.dim() != 2 or t.dim() != 1 or x.shape[1] != p.shape[1] or t.shape[0] != x.shape[0]:
+        raise RuntimeError("mgproto_b200: proxy_anchor takes embeddings [B, E], proxies [C, E] and labels [B], got %s, "
+                           "%s, %s" % (tuple(x.shape), tuple(p.shape), tuple(t.shape)))
+    (B, E), C = x.shape, p.shape[0]
+    loss = torch.empty((1,), device=x.device, dtype=torch.float32)
+    n_valid = torch.empty((1,), device=x.device, dtype=torch.int32)
+    gx = torch.empty_like(x) if want_gx else None
+    gp = torch.empty_like(p) if want_gp else None
+    check(_lib.load().mgp_proxy_anchor(x.data_ptr(), code, p.data_ptr(), t.data_ptr(), B, C, E, float(margin),
+                                       float(beta), loss.data_ptr(), _p(gx), _p(gp), n_valid.data_ptr(), _stream()),
+          "mgp_proxy_anchor")
+    _count(1)
+    return loss, gx, gp, n_valid
+
+
+class ProxyAnchorFunction(torch.autograd.Function):
+    """The Proxy-Anchor criterion (ref utils/losses.py:29-61) with value and both gradients from one kernel: backward
+    only scales the saved gradients by the incoming one, which stays on the device.  An input that does not require
+    a gradient gets a null pointer and its pass is skipped."""
+
+    @staticmethod
+    def forward(ctx, x, proxies, labels, margin, beta):
+        loss, gx, gp, _ = _proxy_anchor(x, proxies, labels, margin, beta, ctx.needs_input_grad[0],
+                                        ctx.needs_input_grad[1])
+        ctx.save_for_backward(gx, gp)
+        return loss.reshape(())
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g):
+        gx, gp = ctx.saved_tensors
+        return (None if gx is None else (gx * g).to(gx.dtype), None if gp is None else gp * g, None, None, None)
+
+
+def proxy_anchor(x, proxies, labels, margin=0.1, beta=32.0):
+    """loss (0-dim fp32) of embeddings x [B,E] (fp32 / bf16 / fp16) against proxies [C,E] (fp32) for labels [B] (int64;
+    a label outside [0, C) takes the image out of every sum).  Differentiable in x and proxies; under torch.no_grad()
+    (evaluation) no gradient pass runs."""
+    if not torch.is_grad_enabled():
+        return _proxy_anchor(x, proxies, labels, float(margin), float(beta), False, False)[0].reshape(())
+    return ProxyAnchorFunction.apply(x, proxies, labels, float(margin), float(beta))
