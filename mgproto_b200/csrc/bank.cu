@@ -11,11 +11,11 @@
 #include <cuda_fp16.h>
 
 #include "mgp_common.cuh"
+#include "tc_ptx.cuh"
 
 namespace {
 
-// fp16 hi / lo split of 256 x (22 mantissa bits; the factor keeps the lo part in fp16's normal range for unit-norm
-// rows) + |x|^2: the tensor-core EM kernel (em_tc.cu) TMA-loads these tiles instead of converting fp32 rows on chip.
+// fp16 hi / lo split of X_SCALE x (tc_ptx.cuh) + |x|^2: the tensor-core EM kernel (em_tc.cu) TMA-loads these tiles instead of converting fp32 rows on chip.
 __device__ __forceinline__ void shadow_store_row(const float* __restrict__ src, __half* __restrict__ xh,
                                                  __half* __restrict__ xl, float* __restrict__ xx, size_t row, int D,
                                                  int lane) {
@@ -27,9 +27,7 @@ __device__ __forceinline__ void shadow_store_row(const float* __restrict__ src, 
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
             ss = fmaf(a[i], a[i], ss);
-            const float s1 = a[i] * 256.0f;
-            h[i] = __float2half_rn(s1);
-            l[i] = __float2half_rn(s1 - __half2float(h[i]));
+            mgp_tc::split_f16(a[i] * mgp_tc::X_SCALE, h[i], l[i]);
         }
         *reinterpret_cast<uint2*>(xh + row * D + 4 * d4) = *reinterpret_cast<uint2*>(h);
         *reinterpret_cast<uint2*>(xl + row * D + 4 * d4) = *reinterpret_cast<uint2*>(l);

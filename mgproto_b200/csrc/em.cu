@@ -1619,9 +1619,8 @@ extern "C" int mgp_em_estep(const float* x, const float* mu, const float* sigma,
     if (K > 64 || (D % 4) != 0 || D > 512) return MGP_ERR_UNSUPPORTED;
     const size_t smem = ((size_t)2 * K * D + K) * sizeof(float);
     if (smem > 220 * 1024) return MGP_ERR_UNSUPPORTED;
-    int dev = 0, sms = 0;
-    MGP_CUDA(cudaGetDevice(&dev));
-    MGP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    int sms = 0;
+    MGP_CUDA(mgp_sm_count(&sms));
     int grid = (n + 7) / 8;
     if (grid > sms * 8) grid = sms * 8;
     cudaStream_t st = (cudaStream_t)stream;

@@ -46,7 +46,6 @@ namespace {
 using namespace mgp_em;
 using namespace mgp_tc;
 
-constexpr float SX = 256.0f;      // shadow rows hold 256 x (fp16 hi + lo)
 constexpr float SR = 1024.0f;     // responsibilities are stored as 1024 r
 constexpr int S1_STRIDE = 17;     // S1 hand-over [D][17] fp32 (padded against bank conflicts)
 
@@ -408,11 +407,9 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
                     if (k < K) {
                         const float r = rr_v[h][rr][q];
                         s0v[q] += r;
-                        const float rs = r * SR;
-                        const __half hh = __float2half_rn(rs);
                         const uint32_t off = rbase + (uint32_t)k * 128u + (uint32_t)(((c16 ^ (k & 7)) & 7) << 4);
-                        *reinterpret_cast<__half*>(rbp + off) = hh;                                          // row k
-                        *reinterpret_cast<__half*>(rbp + off + 2048u) = __float2half_rn(rs - __half2float(hh));   // row 16 + k
+                        split_f16(r * SR, *reinterpret_cast<__half*>(rbp + off),                  // row k
+                                  *reinterpret_cast<__half*>(rbp + off + 2048u));                 // row 16 + k
                     }
                 }
             }
@@ -523,18 +520,16 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
 #pragma unroll
         for (int k = 0; k < KT; ++k)
             if (own && k < K) {
-                const float a = -2.0f * s_w[k] * p_[k] * a_scale;
-                const __half h = __float2half_rn(a);
                 const uint32_t off = (uint32_t)(tid >> 6) * 4096u + (uint32_t)k * 128u +
                                      (uint32_t)(((((tid & 63) >> 3) ^ (k & 7)) & 7) << 4) + (uint32_t)(tid & 7) * 2u;
-                *reinterpret_cast<__half*>(bp + o_a + off) = h;                                   // row k      (hi)
-                *reinterpret_cast<__half*>(bp + o_a + off + 2048u) = __float2half_rn(a - __half2float(h));   // row 16 + k (lo): same swizzle phase
+                split_f16(-2.0f * s_w[k] * p_[k] * a_scale, *reinterpret_cast<__half*>(bp + o_a + off),   // row k      (hi)
+                          *reinterpret_cast<__half*>(bp + o_a + off + 2048u));   // row 16 + k (lo): same swizzle phase
             }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // operand stores -> visible to the MMA (async proxy)
         __syncthreads();
 
         float s0v[4] = {0.f, 0.f, 0.f, 0.f};                          // warps 0-3: S0 of components 8 (q / 2) + 2 t4 + q % 2
-        const float inv_a = 1.0f / (a_scale * SX);
+        const float inv_a = 1.0f / (a_scale * X_SCALE);
 
         if constexpr (WG1) {
             // xfull[s]: a tile landed in slot s.  Tile g of the class's timeline (row tile g % ntiles of loop
@@ -644,7 +639,7 @@ em_tc_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ 
                 newp[k] = p_[k];
                 if (k < K) {
                     const float muv = p_[k];
-                    const float s1 = sacc[k] * (1.0f / (SX * SR));
+                    const float s1 = sacc[k] * (1.0f / (X_SCALE * SR));
                     float g = -(s1 - muv * s_s0[k]) * s_w[k] / n_rows;
                     float esum = 0.f, emu = 0.f;
 #pragma unroll

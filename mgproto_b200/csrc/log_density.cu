@@ -3,10 +3,10 @@
 //   logp_c[b,c,hw] = logsumexp_k( lp_ck(x_n) + log(pi_ck + 1e-10) ),   lp with eps = 1e-10 in (sigma + eps), log(sigma + eps)
 //   logp_all[b,hw] = logsumexp_c logp_c[b,c,hw]                         (per-patch log sum_c p(x|c))
 //
-// Tensor-core path (isotropic sigma, D in {64, 128}, K <= 64): the log-likelihood GEMM of logprob_tcz.cu -- fp32 patch
-// tiles TMA-loaded and split in registers into the fp16 hi / lo A fragments of wgmma (RS form), prototype tiles from the
-// cached pre-pass operands of logprob_tc.cu through a TMA / mbarrier ring, hi*hi + lo*hi + hi*lo in fp32 accumulators --
-// with a new epilogue: nothing of [N,P] leaves the SM.
+// Tensor-core path (isotropic sigma, D in {64, 128}, K <= 64): the log-likelihood GEMM of logprob_tcz.cu, from the same
+// mainloop (tc_rs_gemm.cuh: fp32 patch tiles split in registers into the fp16 hi / lo A fragments of wgmma, prototype
+// tiles from the cached pre-pass operands of logprob_tc.cu through a TMA / mbarrier ring) with its own schedule and
+// epilogue: nothing of [N,P] leaves the SM.
 //   * class-aligned prototype tiles: tile t holds classes [t cpt, (t+1) cpt), cpt = floor(128 / K), i.e. the first
 //     cpt K of the 128 MMA columns; the columns behind them (the next tile's classes, or zero fill past P) are computed
 //     and ignored, so a class never straddles two tiles;
@@ -27,18 +27,14 @@
 
 #include "mgp_common.cuh"
 #include "tc_ptx.cuh"
+#include "tc_rs_gemm.cuh"
 
 namespace {
 using namespace mgp_tc;
+using namespace mgp_rs;
 
-constexpr int LT = 320;            // threads: warps 0-7 two consumer warpgroups, 8 prototype TMA, 9 patch-tile TMA
-constexpr int PT = 128;            // MMA columns per prototype tile (wgmma N)
-constexpr int XT = 128;            // patches per x tile (two warpgroups x m64)
-constexpr int KB = 64;             // K elements per prototype smem block (128 B rows)
-constexpr int PSUB = PT * KB * 2;  // one [128 x 64] fp16 block = 16 KiB
 constexpr int RP = 68;             // pitch (floats) of the reduction tile [PT prototypes][64 patches]: 2 t RP = 8 t mod 32
 constexpr uint32_t RED_BYTES = PT * RP * 4;
-constexpr float X_SCALE = 256.0f;
 constexpr float PI_EPS = 1e-10f;   // ref model.py:415 torch.log(pi + eps)
 constexpr long long FALLBACK_CHUNK_FLOATS = 16ll << 20;   // [n, P] rows of the fallback: at most 64 MiB per chunk
 
@@ -54,10 +50,6 @@ struct LdParams {
     int n_xtiles, n_ptiles;
     int stages;                    // prototype ring depth
 };
-
-__device__ __forceinline__ uint32_t pack_h2(__half a, __half b) {
-    return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
-}
 
 // (M, S) stands for M + log S; merge the partial (m, s) into it
 __device__ __forceinline__ void lse_merge(float& M, float& S, float m, float s) {
@@ -75,25 +67,10 @@ __device__ __forceinline__ float lse_value(float m, float s) { return m == -INFI
 template <int D>
 __device__ __forceinline__ void log_density_tc_body(const CUtensorMap* map_x, const CUtensorMap* map_ph,
                                                     const CUtensorMap* map_pl, const LdParams& prm) {
-    constexpr int NKB = D / KB;                    // prototype K blocks per tile
-    constexpr int NKS = D / 16;                    // k16 steps
-    constexpr int NXB = D / 32;                    // fp32 landing blocks of [128 rows x 32 floats] (128 B rows, swizzled)
-    constexpr uint32_t XB_BYTES = XT * 128;
-    constexpr uint32_t X_BYTES = NXB * XB_BYTES;
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t raw = smem_u32(smem_raw);
-    const uint32_t base = (raw + 1023u) & ~1023u;
-    uint8_t* bp = smem_raw + (base - raw);
     const int S = prm.stages;
-    const uint32_t o_x = 0;                                    // fp32 landing tile
-    const uint32_t o_ring = X_BYTES;                           // S x (proto hi, proto lo)
-    const uint32_t o_red = o_ring + (uint32_t)S * 2 * PSUB;    // two reduction tiles, one per warpgroup
-    const uint32_t o_misc = o_red + 2 * RED_BYTES;             // barriers, then the row partials
-    const uint32_t bar0 = base + o_misc;                       // full[8] empty[8] xfull xempty
-    auto FULL = [&](int i) { return bar0 + 8u * i; };
-    auto EMPTY = [&](int i) { return bar0 + 8u * (8 + i); };
-    const uint32_t XFULL = bar0 + 8u * 16, XEMPTY = bar0 + 8u * 17;
-    float2* s_part = reinterpret_cast<float2*>(bp + o_misc + 256);   // [2 warpgroups][64 patches] (max, sum)
+    const RsSmem<D> sm(S, 2 * RED_BYTES);                      // epilogue region: two reduction tiles, one per warpgroup
+    // behind the barriers: the row partials [2 warpgroups][64 patches] (max, sum)
+    float2* s_part = reinterpret_cast<float2*>(sm.epi() + 2 * RED_BYTES + 256);
 
     if (*reinterpret_cast<const volatile int*>(prm.noniso) != 0) {
         // the caller asserted isotropic sigma and the prototype pre-pass found otherwise: NaN outputs, no fault
@@ -106,13 +83,7 @@ __device__ __forceinline__ void log_density_tc_body(const CUtensorMap* map_x, co
     }
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < 8; ++i) { mbar_init(FULL(i), 1); mbar_init(EMPTY(i), 8); }   // empty: one arrive per consumer warp
-        mbar_init(XFULL, 1);
-        mbar_init(XEMPTY, 8);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
+    init_barriers(sm);
 
     // x-stationary schedule: x tiles blockIdx.x, blockIdx.x + grid, ...; every prototype tile against each
     const int n_my_x = blockIdx.x < prm.n_xtiles ? (prm.n_xtiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
@@ -122,34 +93,17 @@ __device__ __forceinline__ void log_density_tc_body(const CUtensorMap* map_x, co
     if (n_my_x == 0) {
         // nothing to do for this CTA
     } else if (warp == 9 && lane == 0) {
-        // =========================== fp32 patch-tile producer (the next tile lands under the current one's MMAs) =====
-        for (int c = 0; c < n_my_x; ++c) {
-            if (c > 0) mbar_wait(XEMPTY, (uint32_t)((c - 1) & 1));   // the consumers converted the previous tile
-            mbar_expect_tx(XFULL, X_BYTES);
-            const int xt = blockIdx.x + c * gridDim.x;
-#pragma unroll
-            for (int b = 0; b < NXB; ++b) tma_load_2d(base + o_x + b * XB_BYTES, map_x, b * 32, xt * XT, XFULL);
-        }
+        produce_x_tiles(sm, map_x, n_my_x, [](int c) { return (int)(blockIdx.x + c * gridDim.x); });
     } else if (warp == 8 && lane == 0) {
-        // =========================== prototype TMA producer: 128 rows from the first row of the tile's classes =====
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int c = 0; c < n_my_x; ++c)
-            for (int pt = 0; pt < n_ptiles; ++pt)
-                for (int kb = 0; kb < NKB; ++kb) {
-                    mbar_wait(EMPTY(stage), phase ^ 1u);
-                    mbar_expect_tx(FULL(stage), 2 * PSUB);
-                    const uint32_t dst = base + o_ring + (uint32_t)stage * 2 * PSUB;
-                    tma_load_2d(dst, map_ph, D + kb * KB, pt * tile_rows, FULL(stage));   // the [-2 w mu] half of [P, 2D]
-                    tma_load_2d(dst + PSUB, map_pl, D + kb * KB, pt * tile_rows, FULL(stage));
-                    if (++stage == S) { stage = 0; phase ^= 1u; }
-                }
+        // 128 rows from the first row of the tile's classes
+        produce_proto_tiles(sm, map_ph, map_pl, S, n_my_x, [](int) { return 0; }, [&](int) { return n_ptiles; },
+                            [&](int pt) { return pt * tile_rows; });
     } else if (warp < 8) {
         // =========================== consumers: split, MMA, class log-sum-exp ===========================
         const int wg = warp >> 2, wq = warp & 3, g = lane >> 2, t = lane & 3;
         const int rA = wg * 64 + wq * 16 + g;                    // this thread's fragment rows of the tile: rA, rA + 8
         const int u = threadIdx.x & 127, rr = u & 63, par = u >> 6;   // reduction role: patch rr of the slice, classes par + 2 j
-        float* red = reinterpret_cast<float*>(bp + o_red + (uint32_t)wg * RED_BYTES);
+        float* red = reinterpret_cast<float*>(sm.epi() + (uint32_t)wg * RED_BYTES);
         const uint32_t wg_bar = 2 + wg;
         auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(wg_bar) : "memory"); };
         const int C = prm.C, HW = prm.HW;
@@ -157,28 +111,9 @@ __device__ __forceinline__ void log_density_tc_body(const CUtensorMap* map_x, co
         uint32_t phase = 0;
         for (int c = 0; c < n_my_x; ++c) {
             const int row0 = (blockIdx.x + c * gridDim.x) * XT;
-            // ---- fused operand split: fp32 landing tile -> A fragments (hi, lo of 256 x) + |x|^2 of rows rA, rA + 8
-            uint32_t ah[NKS][4], al[NKS][4];
-            float ssA = 0.f, ssB = 0.f;
-            mbar_wait(XFULL, (uint32_t)(c & 1));
-#pragma unroll
-            for (int ks = 0; ks < NKS; ++ks) {
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {                    // fragment register q: row rA + 8 (q & 1), k 16 ks + 2 t + 8 (q >> 1)
-                    const int r = rA + 8 * (q & 1), col = 16 * ks + 2 * t + 8 * (q >> 1), w = col & 31;
-                    const float2 v = *reinterpret_cast<const float2*>(
-                        bp + o_x + (uint32_t)(col >> 5) * XB_BYTES + (uint32_t)r * 128u + ((((w >> 2) ^ (r & 7)) & 7) << 4) + (w & 3) * 4);
-                    if (q & 1) ssB = fmaf(v.x, v.x, fmaf(v.y, v.y, ssB)); else ssA = fmaf(v.x, v.x, fmaf(v.y, v.y, ssA));
-                    const float s0 = v.x * X_SCALE, s1 = v.y * X_SCALE;
-                    const __half h0 = __float2half_rn(s0), h1 = __float2half_rn(s1);
-                    ah[ks][q] = pack_h2(h0, h1);
-                    al[ks][q] = pack_h2(__float2half_rn(s0 - __half2float(h0)), __float2half_rn(s1 - __half2float(h1)));
-                }
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(XEMPTY);                  // landing tile consumed: the next one may land
-            ssA += __shfl_xor_sync(0xffffffffu, ssA, 1); ssA += __shfl_xor_sync(0xffffffffu, ssA, 2);
-            ssB += __shfl_xor_sync(0xffffffffu, ssB, 1); ssB += __shfl_xor_sync(0xffffffffu, ssB, 2);
+            uint32_t ah[RsSmem<D>::NKS][4], al[RsSmem<D>::NKS][4];
+            float ssA, ssB;
+            split_x_tile(sm, c, rA, lane, ah, al, ssA, ssB);
 
             const int n = row0 + wg * 64 + rr;                   // the patch this thread reduces
             const bool nok = n < prm.N;
@@ -186,26 +121,7 @@ __device__ __forceinline__ void log_density_tc_body(const CUtensorMap* map_x, co
             float run_m = -INFINITY, run_s = 0.f;                // over the classes par, par + 2, ... of every tile
             for (int pt = 0; pt < n_ptiles; ++pt) {
                 float acc[64];
-#pragma unroll
-                for (int j = 0; j < 64; ++j) acc[j] = 0.f;
-                for (int kb = 0; kb < NKB; ++kb) {
-                    mbar_wait(FULL(stage), phase);
-                    const uint32_t ph = base + o_ring + (uint32_t)stage * 2 * PSUB, pl = ph + PSUB;
-                    wg_fence();
-#pragma unroll
-                    for (int k = 0; k < KB / 16; ++k) {
-                        const int ks = (kb * KB) / 16 + k;
-                        const uint64_t b_h = gmma_desc(ph + (uint32_t)k * 32u), b_l = gmma_desc(pl + (uint32_t)k * 32u);
-                        wg_mma_rs_n128(acc, ah[ks], b_h);
-                        wg_mma_rs_n128(acc, al[ks], b_h);
-                        wg_mma_rs_n128(acc, ah[ks], b_l);
-                    }
-                    wg_commit();
-                    wg_wait0();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(EMPTY(stage));    // this warp no longer reads the stage
-                    if (++stage == S) { stage = 0; phase ^= 1u; }
-                }
+                mma_proto_tile(sm, acc, ah, al, S, lane, stage, phase);
                 const int cls0 = pt * prm.cpt;
                 const int ncls = min(prm.cpt, C - cls0);
                 const int ncol = ncls * K, p0 = cls0 * K;
@@ -252,13 +168,13 @@ __device__ __forceinline__ void log_density_tc_body(const CUtensorMap* map_x, co
     }
 }
 
-__global__ void __launch_bounds__(LT, 1)
+__global__ void __launch_bounds__(RS_THREADS, 1)
 log_density_tc_d64_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_ph,
                           const __grid_constant__ CUtensorMap map_pl, const LdParams prm) {
     log_density_tc_body<64>(&map_x, &map_ph, &map_pl, prm);
 }
 
-__global__ void __launch_bounds__(LT, 1)
+__global__ void __launch_bounds__(RS_THREADS, 1)
 log_density_tc_d128_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_ph,
                            const __grid_constant__ CUtensorMap map_pl, const LdParams prm) {
     log_density_tc_body<128>(&map_x, &map_ph, &map_pl, prm);
@@ -304,20 +220,6 @@ __global__ void log_density_lse_kernel(const float* __restrict__ lp, const float
         if (lane == 0) out_bhw[n] = lse_value(M, S);
     }
 }
-
-bool make_map_x(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols) {
-    EncodeTiledFn enc = get_encode();
-    if (!enc) return false;
-    cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {cols * 4};
-    cuuint32_t box[2] = {32, XT};
-    cuuint32_t es[2] = {1, 1};
-    return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(ptr), dims, strides, box, es,
-               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 
 bool tc_shape(int K, int D) { return (D == 64 || D == 128) && K >= 1 && K <= 64 && get_encode() != nullptr; }
 bool tc_math(int math) { return math == MGP_MATH_TC_ISO || math == MGP_MATH_TC_ISO_REUSE; }
@@ -390,23 +292,17 @@ extern "C" int mgp_log_density(const float* xhat_nd, const float* mu, const floa
         prm.cpt = PT / K;
         prm.n_xtiles = (int)((N + XT - 1) / XT);
         prm.n_ptiles = (C + prm.cpt - 1) / prm.cpt;
-        int dev = 0, sms = 0;
-        MGP_CUDA(cudaGetDevice(&dev));
-        MGP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-        const size_t x_bytes = (size_t)XT * D * 4, fixed = 1024 + x_bytes + 2 * RED_BYTES + 256 + 2 * 64 * 8;
-        const size_t smem_max = 227 * 1024;
-        int stages = (int)((smem_max - fixed) / (2 * PSUB));
-        if (stages > 8) stages = 8;
-        if (stages < 2) return MGP_ERR_UNSUPPORTED;
-        prm.stages = stages;
-        const size_t smem = fixed + (size_t)stages * 2 * PSUB;
+        int sms = 0;
+        MGP_CUDA(mgp_sm_count(&sms));
+        size_t smem;
+        if (!rs_smem_plan(D, 2 * RED_BYTES + 2 * 64 * 8, &prm.stages, &smem)) return MGP_ERR_UNSUPPORTED;
         const int grid = prm.n_xtiles < sms ? prm.n_xtiles : sms;
         if (D == 64) {
             MGP_CUDA(cudaFuncSetAttribute(log_density_tc_d64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            log_density_tc_d64_kernel<<<grid, LT, smem, st>>>(mx, mph, mpl, prm);
+            log_density_tc_d64_kernel<<<grid, RS_THREADS, smem, st>>>(mx, mph, mpl, prm);
         } else {
             MGP_CUDA(cudaFuncSetAttribute(log_density_tc_d128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            log_density_tc_d128_kernel<<<grid, LT, smem, st>>>(mx, mph, mpl, prm);
+            log_density_tc_d128_kernel<<<grid, RS_THREADS, smem, st>>>(mx, mph, mpl, prm);
         }
         MGP_CHECK_LAUNCH();
         return MGP_OK;

@@ -47,7 +47,6 @@ constexpr int STAGING_BYTES = 8 * 32 * 32 * 4;   // one [32 x 32] fp32 block per
 constexpr int PT = 128;          // prototypes per tile (two warpgroups x 64)
 constexpr int KB = 64;           // K elements per smem block (128 B rows, SWIZZLE_128B)
 constexpr int SUB_BYTES = 128 * KB * 2;   // one [128 x 64] fp16 block = 16 KiB
-constexpr float X_SCALE = 256.0f;
 
 // ------------------------------------------------------------------------------------------ PTX (tc_ptx.cuh)
 using namespace mgp_tc;
@@ -88,11 +87,8 @@ __global__ void tc_proto_prep_kernel(const float* __restrict__ mu, const float* 
         const float r = 1.0f / (sr[d] + eps);
         const float w = r * r;
         const float v0 = w * scale, v1 = -2.0f * w * mr[d] * scale;
-        const __half h0 = __float2half_rn(v0), h1 = __float2half_rn(v1);
-        bh[(size_t)p * 2 * D + d] = h0;
-        bl[(size_t)p * 2 * D + d] = __float2half_rn(v0 - __half2float(h0));
-        bh[(size_t)p * 2 * D + D + d] = h1;
-        bl[(size_t)p * 2 * D + D + d] = __float2half_rn(v1 - __half2float(h1));
+        split_f16(v0, bh[(size_t)p * 2 * D + d], bl[(size_t)p * 2 * D + d]);
+        split_f16(v1, bh[(size_t)p * 2 * D + D + d], bl[(size_t)p * 2 * D + D + d]);
     }
     if (lane == 0) {
         const float r0 = 1.0f / (s0 + eps);
@@ -122,12 +118,8 @@ __global__ void tc_x_prep_kernel(const float* __restrict__ x, __half* __restrict
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
             ss = fmaf(a[i], a[i], ss);
-            const float s1 = a[i] * X_SCALE;
-            h[i] = __float2half_rn(s1);
-            l[i] = __float2half_rn(s1 - __half2float(h[i]));
-            const float s2 = a[i] * a[i] * X_SCALE;
-            h2[i] = __float2half_rn(s2);
-            l2[i] = __float2half_rn(s2 - __half2float(h2[i]));
+            split_f16(a[i] * X_SCALE, h[i], l[i]);
+            split_f16(a[i] * a[i] * X_SCALE, h2[i], l2[i]);
         }
         *reinterpret_cast<uint2*>(hr + D + d4 * 4) = *reinterpret_cast<uint2*>(h);
         *reinterpret_cast<uint2*>(lr + D + d4 * 4) = *reinterpret_cast<uint2*>(l);
@@ -704,11 +696,6 @@ logprob_top1_wide_kernel(const __grid_constant__ CUtensorMap map_xh, const __gri
 }
 
 // ------------------------------------------------------------------------------------------ host
-// [rows, cols] fp16 row-major, box = 64 cols x box_rows, 128 B swizzle; OOB rows read as zero (tc_ptx.cuh)
-bool make_map(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows) {
-    return make_map_f16(m, ptr, rows, cols, box_rows);
-}
-
 // output [N, P] fp32 row-major, box = 32 prototypes x 32 patches, no swizzle (TMA-store epilogue)
 bool make_out_map(CUtensorMap* m, const void* ptr, uint64_t N, uint64_t P) {
     EncodeTiledFn enc = get_encode();
@@ -734,8 +721,6 @@ bool make_out_map_bphw(CUtensorMap* m, const void* ptr, uint64_t B, uint64_t P, 
                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
-
-size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 
 struct WsLayout {
     size_t bh, bl, e0, e1, e2, flag, ah, al, sn, total;
@@ -857,8 +842,8 @@ int mgp_logprob_tc_launch(const float* xhat, const float* mu, const float* sigma
     const bool img_tiles = tma_bphw && !top1;
     const uint32_t xbox = img_tiles ? 32u : 128u;
     if (top1_tiles) MGP_CUDA(cudaMemsetAsync(out, 0, (size_t)B * P * sizeof(unsigned long long), st));
-    if (!make_map(&mxh, ah, (uint64_t)N, 2 * D, xbox) || !make_map(&mxl, al, (uint64_t)N, 2 * D, xbox) ||
-        !make_map(&mph, bh, (uint64_t)P, 2 * D, 128) || !make_map(&mpl, bl, (uint64_t)P, 2 * D, 128))
+    if (!make_map_f16(&mxh, ah, (uint64_t)N, 2 * D, xbox) || !make_map_f16(&mxl, al, (uint64_t)N, 2 * D, xbox) ||
+        !make_map_f16(&mph, bh, (uint64_t)P, 2 * D, 128) || !make_map_f16(&mpl, bl, (uint64_t)P, 2 * D, 128))
         return MGP_ERR_UNSUPPORTED;
     if (tma_bphw && !top1) {
         if (!make_out_map_bphw(&mout, out, (uint64_t)B, (uint64_t)P, (uint64_t)HW)) return MGP_ERR_UNSUPPORTED;
@@ -880,9 +865,8 @@ int mgp_logprob_tc_launch(const float* xhat, const float* mu, const float* sigma
     prm.B = B;
     prm.xbox = (int)xbox;
     prm.nti = ((HW + 31) / 32) * 32;
-    int dev = 0, sms = 0;
-    MGP_CUDA(cudaGetDevice(&dev));
-    MGP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    int sms = 0;
+    MGP_CUDA(mgp_sm_count(&sms));
     // teams of 4 CTAs (fewer when there are fewer prototype tiles) share an x tile and write adjacent tiles
     int team = 4;
     {
@@ -900,7 +884,7 @@ int mgp_logprob_tc_launch(const float* xhat, const float* mu, const float* sigma
         // the x map's box is the whole image tile (NI rows, NI = HW rounded up to an instantiated width)
         const int ni = HW <= 32 ? 32 : HW <= 56 ? 56 : HW <= 64 ? 64 : HW <= 128 ? 128 : HW <= 200 ? 200 : 256;
         CUtensorMap wxh, wxl;
-        if (!make_map(&wxh, ah, (uint64_t)N, 2 * D, (uint32_t)ni) || !make_map(&wxl, al, (uint64_t)N, 2 * D, (uint32_t)ni))
+        if (!make_map_f16(&wxh, ah, (uint64_t)N, 2 * D, (uint32_t)ni) || !make_map_f16(&wxl, al, (uint64_t)N, 2 * D, (uint32_t)ni))
             return MGP_ERR_UNSUPPORTED;
         TcParams pw = prm;
         pw.iso_elsewhere = iso_known ? 0 : 1;

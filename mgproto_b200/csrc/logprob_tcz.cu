@@ -2,12 +2,11 @@
 //
 // logprob_tc.cu feeds both operands of every MMA from shared memory and needs a separate pass that splits x into fp16
 // hi/lo operands in HBM (25.7 MB read, 2 x 25.7 MB written and read back at cfg2).  Here:
-//   * the fp32 patch tile [128 x D] is TMA-loaded as it is (no operand pre-pass over x: the split is fused); each of the
-//     two consumer warpgroups converts its 64-patch slice in registers to fp16 hi / lo of 256 x, laid out as the A
-//     fragments of wgmma.mma_async (RS form), where they stay for the 3 * D/16 MMAs of every prototype tile the CTA
-//     visits with this x tile; |x|^2 of the rank-1 epilogue term is summed in the same pass;
-//   * only the prototype tiles (B operand, the small side: 2 * P * D * 2 bytes in total, L2-resident) stream through a
-//     TMA / mbarrier ring in shared memory; the next fp32 patch tile lands under the current one's MMAs;
+//   * the GEMM is the register-operand mainloop of tc_rs_gemm.cuh (shared with log_density.cu): the fp32 patch tile
+//     [128 x D] is TMA-loaded as it is and split in registers into the fp16 hi / lo A fragments of wgmma (RS form), so
+//     there is no operand pre-pass over x; they stay for the 3 * D/16 MMAs of every prototype tile the CTA visits with
+//     this x tile; only the prototype tiles (B operand, the small side: 2 * P * D * 2 bytes in total, L2-resident)
+//     stream through a TMA / mbarrier ring in shared memory;
 //   * accumulator rows are patches and columns prototypes, so the fragments of a warp are 16 consecutive output rows:
 //     they go, with the affine fix-up, into 128B-swizzled [16 rows x 32 floats] blocks (conflict-free float2 stores)
 //     and out through asynchronous TMA bulk tensor stores (plain stores from the row owners if P % 4 != 0);
@@ -24,17 +23,13 @@
 
 #include "mgp_common.cuh"
 #include "tc_ptx.cuh"
+#include "tc_rs_gemm.cuh"
 
 namespace {
 using namespace mgp_tc;
+using namespace mgp_rs;
 
-constexpr int ZT = 320;            // threads
-constexpr int PT = 128;            // prototypes per tile (wgmma N)
-constexpr int XT = 128;            // patches per tile (two warpgroups x m64)
-constexpr int KB = 64;             // K elements per prototype smem block (128 B rows)
-constexpr int PSUB = PT * KB * 2;  // one [128 x 64] fp16 block = 16 KiB
 constexpr int STG = 2048;          // one [16 rows x 32 floats] output block; two per consumer warp
-constexpr float X_SCALE = 256.0f;
 
 struct ZParams {
     const float* e0;
@@ -47,42 +42,15 @@ struct ZParams {
     int stages;                    // prototype ring depth
 };
 
-__device__ __forceinline__ uint32_t pack_h2(__half a, __half b) {
-    return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
-}
-
 template <int D>
-__global__ void __launch_bounds__(ZT, 1)
+__global__ void __launch_bounds__(RS_THREADS, 1)
 logprob_z_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_ph,
                  const __grid_constant__ CUtensorMap map_pl, const __grid_constant__ CUtensorMap map_out,
                  const ZParams prm) {
-    constexpr int NKB = D / KB;                    // prototype K blocks per tile
-    constexpr int NKS = D / 16;                    // k16 steps
-    constexpr int NXB = D / 32;                    // fp32 landing blocks of [128 rows x 32 floats] (128 B rows, swizzled)
-    constexpr uint32_t XB_BYTES = XT * 128;        // 16 KiB
-    constexpr uint32_t X_BYTES = NXB * XB_BYTES;
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t raw = smem_u32(smem_raw);
-    const uint32_t base = (raw + 1023u) & ~1023u;
-    uint8_t* bp = smem_raw + (base - raw);
     const int S = prm.stages;
-    const uint32_t o_x = 0;                                    // fp32 landing tile
-    const uint32_t o_ring = X_BYTES;                           // S x (proto hi, proto lo)
-    const uint32_t o_stg = o_ring + (uint32_t)S * 2 * PSUB;    // 8 warps x 2 output blocks
-    const uint32_t o_misc = o_stg + 8 * 2 * STG;
-    const uint32_t bar0 = base + o_misc;                       // full[8] empty[8] xfull xempty
-    auto FULL = [&](int i) { return bar0 + 8u * i; };
-    auto EMPTY = [&](int i) { return bar0 + 8u * (8 + i); };
-    const uint32_t XFULL = bar0 + 8u * 16, XEMPTY = bar0 + 8u * 17;
-
+    const RsSmem<D> sm(S, 8 * 2 * STG);                       // epilogue region: 8 warps x 2 output blocks
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < 8; ++i) { mbar_init(FULL(i), 1); mbar_init(EMPTY(i), 8); }   // empty: one arrive per consumer warp
-        mbar_init(XFULL, 1);
-        mbar_init(XEMPTY, 8);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
+    init_barriers(sm);
 
     const int n_ptiles = prm.n_ptiles;
     const long long n_pairs = (long long)prm.n_xtiles * n_ptiles;
@@ -95,27 +63,9 @@ logprob_z_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
     if (n_my_x == 0) {
         // nothing to do for this CTA (tiny problems)
     } else if (warp == 9 && lane == 0) {
-        // =========================== fp32 patch-tile producer (the next tile lands under the current one's MMAs) =====
-        for (int c = 0; c < n_my_x; ++c) {
-            if (c > 0) mbar_wait(XEMPTY, (uint32_t)((c - 1) & 1));   // the consumers converted the previous tile
-            mbar_expect_tx(XFULL, X_BYTES);
-#pragma unroll
-            for (int b = 0; b < NXB; ++b) tma_load_2d(base + o_x + b * XB_BYTES, &map_x, b * 32, (xt_first + c) * XT, XFULL);
-        }
+        produce_x_tiles(sm, &map_x, n_my_x, [&](int c) { return xt_first + c; });
     } else if (warp == 8 && lane == 0) {
-        // =========================== prototype TMA producer ===========================
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int c = 0; c < n_my_x; ++c)
-            for (int pt = p_begin(c); pt < p_end(c); ++pt)
-                for (int kb = 0; kb < NKB; ++kb) {
-                    mbar_wait(EMPTY(stage), phase ^ 1u);
-                    mbar_expect_tx(FULL(stage), 2 * PSUB);
-                    const uint32_t dst = base + o_ring + (uint32_t)stage * 2 * PSUB;
-                    tma_load_2d(dst, &map_ph, D + kb * KB, pt * PT, FULL(stage));    // the [-2 w mu] half of [P, 2D]
-                    tma_load_2d(dst + PSUB, &map_pl, D + kb * KB, pt * PT, FULL(stage));
-                    if (++stage == S) { stage = 0; phase ^= 1u; }
-                }
+        produce_proto_tiles(sm, &map_ph, &map_pl, S, n_my_x, p_begin, p_end, [](int pt) { return pt * PT; });
     } else if (warp < 8) {
         // =========================== consumers ===========================
         if (*reinterpret_cast<const volatile int*>(prm.noniso) != 0) __trap();   // the caller asserted isotropic sigma
@@ -126,50 +76,12 @@ logprob_z_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
         uint32_t phase = 0;
         for (int c = 0; c < n_my_x; ++c) {
             const int row0 = (xt_first + c) * XT;
-            // ---- fused operand split: fp32 landing tile -> A fragments (hi, lo of 256 x) + |x|^2 of rows rA, rA + 8
-            uint32_t ah[NKS][4], al[NKS][4];
-            float ssA = 0.f, ssB = 0.f;
-            mbar_wait(XFULL, (uint32_t)(c & 1));
-#pragma unroll
-            for (int ks = 0; ks < NKS; ++ks) {
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {                    // fragment register q: row rA + 8 (q & 1), k 16 ks + 2 t + 8 (q >> 1)
-                    const int r = rA + 8 * (q & 1), col = 16 * ks + 2 * t + 8 * (q >> 1), w = col & 31;
-                    const float2 v = *reinterpret_cast<const float2*>(
-                        bp + o_x + (uint32_t)(col >> 5) * XB_BYTES + (uint32_t)r * 128u + ((((w >> 2) ^ (r & 7)) & 7) << 4) + (w & 3) * 4);
-                    if (q & 1) ssB = fmaf(v.x, v.x, fmaf(v.y, v.y, ssB)); else ssA = fmaf(v.x, v.x, fmaf(v.y, v.y, ssA));
-                    const float s0 = v.x * X_SCALE, s1 = v.y * X_SCALE;
-                    const __half h0 = __float2half_rn(s0), h1 = __float2half_rn(s1);
-                    ah[ks][q] = pack_h2(h0, h1);
-                    al[ks][q] = pack_h2(__float2half_rn(s0 - __half2float(h0)), __float2half_rn(s1 - __half2float(h1)));
-                }
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(XEMPTY);                  // landing tile consumed: the next one may land
-            ssA += __shfl_xor_sync(0xffffffffu, ssA, 1); ssA += __shfl_xor_sync(0xffffffffu, ssA, 2);
-            ssB += __shfl_xor_sync(0xffffffffu, ssB, 1); ssB += __shfl_xor_sync(0xffffffffu, ssB, 2);
+            uint32_t ah[RsSmem<D>::NKS][4], al[RsSmem<D>::NKS][4];
+            float ssA, ssB;
+            split_x_tile(sm, c, rA, lane, ah, al, ssA, ssB);
             for (int pt = p_begin(c); pt < p_end(c); ++pt) {
                 float acc[64];
-#pragma unroll
-                for (int j = 0; j < 64; ++j) acc[j] = 0.f;
-                for (int kb = 0; kb < NKB; ++kb) {
-                    mbar_wait(FULL(stage), phase);
-                    const uint32_t ph = base + o_ring + (uint32_t)stage * 2 * PSUB, pl = ph + PSUB;
-                    wg_fence();
-#pragma unroll
-                    for (int k = 0; k < KB / 16; ++k) {
-                        const int ks = (kb * KB) / 16 + k;
-                        const uint64_t b_h = gmma_desc(ph + (uint32_t)k * 32u), b_l = gmma_desc(pl + (uint32_t)k * 32u);
-                        wg_mma_rs_n128(acc, ah[ks], b_h);
-                        wg_mma_rs_n128(acc, al[ks], b_h);
-                        wg_mma_rs_n128(acc, ah[ks], b_l);
-                    }
-                    wg_commit();
-                    wg_wait0();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(EMPTY(stage));    // this warp no longer reads the stage
-                    if (++stage == S) { stage = 0; phase ^= 1u; }
-                }
+                mma_proto_tile(sm, acc, ah, al, S, lane, stage, phase);
                 // ---- epilogue: log p = e0 + e1 acc + e2 |x|^2, 4 blocks of [16 patches x 32 prototypes] per warp
 #pragma unroll
                 for (int ch = 0; ch < 4; ++ch) {
@@ -182,7 +94,7 @@ logprob_z_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
                         c2 = ok ? __ldg(prm.e2 + p) : 0.f;
                     };
                     if (tma_out) {
-                        uint8_t* stg = bp + o_stg + (uint32_t)(warp * 2 + sbuf) * STG;
+                        uint8_t* stg = sm.epi() + (uint32_t)(warp * 2 + sbuf) * STG;
                         if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");   // this block's previous store has read it
                         __syncwarp();
 #pragma unroll
@@ -230,18 +142,6 @@ logprob_z_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
     }
 }
 
-bool make_map_x(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols) {
-    EncodeTiledFn enc = get_encode();
-    if (!enc) return false;
-    cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {cols * 4};
-    cuuint32_t box[2] = {32, XT};
-    cuuint32_t es[2] = {1, 1};
-    return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(ptr), dims, strides, box, es,
-               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
 // output [N, P] fp32, box = 32 prototypes x 16 patches, 128B swizzle (inner box = 128 B)
 bool make_map_out(CUtensorMap* m, const void* ptr, uint64_t N, uint64_t P) {
     EncodeTiledFn enc = get_encode();
@@ -275,21 +175,16 @@ int mgp_logprob_tcz_launch(const float* xhat, const void* bh, const void* bl, co
     prm.N = (int)N; prm.P = P;
     prm.n_xtiles = (int)((N + XT - 1) / XT);
     prm.n_ptiles = (P + PT - 1) / PT;
-    int dev = 0, sms = 0;
-    MGP_CUDA(cudaGetDevice(&dev));
-    MGP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    const size_t x_bytes = (size_t)XT * D * 4;
-    int stages = (int)((227 * 1024 - 1024 - 256 - 8 * 2 * STG - x_bytes) / (2 * PSUB));
-    if (stages > 8) stages = 8;
-    if (stages < 2) return MGP_ERR_UNSUPPORTED;
-    prm.stages = stages;
+    int sms = 0;
+    MGP_CUDA(mgp_sm_count(&sms));
+    size_t smem;
+    if (!rs_smem_plan(D, 8 * 2 * STG, &prm.stages, &smem)) return MGP_ERR_UNSUPPORTED;
     const long long n_pairs = (long long)prm.n_xtiles * prm.n_ptiles;
     const int grid = (int)(n_pairs < sms ? n_pairs : sms);
-    const size_t smem = 1024 + x_bytes + (size_t)stages * 2 * PSUB + 8 * 2 * STG + 256;
 #define MGP_Z_LAUNCH(DD)                                                                                           \
     do {                                                                                                           \
         MGP_CUDA(cudaFuncSetAttribute(logprob_z_kernel<DD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        logprob_z_kernel<DD><<<grid, ZT, smem, st>>>(mx, mph, mpl, mout, prm);                                     \
+        logprob_z_kernel<DD><<<grid, RS_THREADS, smem, st>>>(mx, mph, mpl, mout, prm);                                     \
     } while (0)
     if (D == 64) MGP_Z_LAUNCH(64);
     else MGP_Z_LAUNCH(128);

@@ -21,6 +21,13 @@
     } while (0)
 
 static inline bool mgp_aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+static inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
+// streaming multiprocessors of the current device
+static inline cudaError_t mgp_sm_count(int* sms) {
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    return e != cudaSuccess ? e : cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev);
+}
 // MGP_X_F32 / _BF16 / _F16, optionally | MGP_X_NHWC
 static inline bool mgp_x_fmt_valid(int f) { return f >= 0 && (f & ~MGP_X_NHWC) <= MGP_X_F16; }
 

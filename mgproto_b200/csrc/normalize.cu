@@ -16,6 +16,7 @@
 // The backward writes g_x in the feature format: the fp32 value is the same in every format and rounded once
 // (round-to-nearest-even) for 16-bit; NCHW goes through the transposing tile, NHWC rows are written directly.
 #include "mgp_common.cuh"
+#include "tc_ptx.cuh"
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -113,7 +114,7 @@ __global__ void __launch_bounds__(256) normalize_fwd_kernel(const T* __restrict_
             for (int d = lane; d < D; d += 32) dst[d] = tile[d * (NT + 1) + r] * inv;
         } else {
             // ... and the operands the tensor-core log-likelihood kernels read (csrc/logprob_tc.cu tc_x_prep_kernel: rows
-            // of [N, 2D] fp16, hi / lo split of 256 * [ x^2 | x ], the x^2 half only on request; sn = |xhat|^2)
+            // of [N, 2D] fp16, hi / lo split of X_SCALE * [ x^2 | x ], the x^2 half only on request; sn = |xhat|^2)
             __half* hr = ah + n * 2 * D;
             __half* lr = al + n * 2 * D;
             float ss = 0.f;
@@ -121,16 +122,8 @@ __global__ void __launch_bounds__(256) normalize_fwd_kernel(const T* __restrict_
                 const float a = tile[d * (NT + 1) + r] * inv;
                 dst[d] = a;
                 ss = fmaf(a, a, ss);
-                const float s1 = a * 256.0f;
-                const __half h = __float2half_rn(s1);
-                hr[D + d] = h;
-                lr[D + d] = __float2half_rn(s1 - __half2float(h));
-                if (stage_aniso) {
-                    const float s2 = a * a * 256.0f;
-                    const __half h2 = __float2half_rn(s2);
-                    hr[d] = h2;
-                    lr[d] = __float2half_rn(s2 - __half2float(h2));
-                }
+                mgp_tc::split_f16(a * mgp_tc::X_SCALE, hr[D + d], lr[D + d]);
+                if (stage_aniso) mgp_tc::split_f16(a * a * mgp_tc::X_SCALE, hr[d], lr[d]);
             }
             ss = warp_sum(ss);
             if (lane == 0) sn[n] = ss;

@@ -2,11 +2,35 @@
 // SASS: wgmma.mma_async -> HGMMA, cp.async.bulk.tensor -> UTMALDG / UTMASTG, mbarrier -> SYNCS.
 #pragma once
 #include <cuda.h>
+#include <cuda_fp16.h>
 #include <stdint.h>
 
 namespace mgp_tc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+// The fp16 operand format of every tensor-core GEMM here: v = hi + lo with hi = fp16(v), lo = fp16(v - hi) (22
+// mantissa bits); products run as hi*hi + lo*hi + hi*lo with fp32 accumulation.  Patch and bank rows are split as
+// X_SCALE x (the factor keeps lo in fp16's normal range for unit-norm rows); whoever consumes such a product divides
+// X_SCALE out again.  Prototype-side operands carry their own power-of-two scales.
+constexpr float X_SCALE = 256.0f;
+
+__device__ __forceinline__ __half split_f16_lo(float v, __half hi) { return __float2half_rn(v - __half2float(hi)); }
+__device__ __forceinline__ void split_f16(float v, __half& hi, __half& lo) {
+    const __half h = __float2half_rn(v);
+    hi = h;
+    lo = split_f16_lo(v, h);
+}
+__device__ __forceinline__ uint32_t pack_h2(__half a, __half b) {
+    return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
+}
+// two consecutive k of an RS A fragment register (the lower k in the low half); both hi halves are packed before the
+// lo halves are formed, which keeps fewer values live in the fully unrolled fragment loops
+__device__ __forceinline__ void split_f16x2(float v0, float v1, uint32_t& hi, uint32_t& lo) {
+    const __half h0 = __float2half_rn(v0), h1 = __float2half_rn(v1);
+    hi = pack_h2(h0, h1);
+    lo = pack_h2(split_f16_lo(v0, h0), split_f16_lo(v1, h1));
+}
 
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));

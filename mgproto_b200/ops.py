@@ -30,6 +30,24 @@ _iso_cache = {}
 
 
 _PROTO_OPERANDS = collections.OrderedDict()   # (mu, sigma identity + version, shape, device, stream) -> (workspace, mu, sigma)
+_DENSITY_OPERANDS = collections.OrderedDict()   # as _PROTO_OPERANDS, for log_density's tensor-core workspace
+
+
+def _cached_operands(cache, key, nbytes):
+    """The workspace that already holds the prototype-side operands for `key` (mu / sigma unchanged), or None."""
+    hit = cache.get(key)
+    if hit is None or hit[0].numel() < nbytes:
+        return None
+    cache.move_to_end(key)
+    return hit[0]
+
+
+def _keep_operands(cache, key, ws, mu, sg):
+    """Remember ws as holding the operands for key; two entries per cache.  The entry keeps mu / sigma alive, so their
+    addresses cannot be recycled under the key."""
+    cache[key] = (ws, mu, sg)
+    while len(cache) > 2:
+        cache.popitem(last=False)
 
 
 def sigma_is_isotropic(sigma: torch.Tensor) -> bool:
@@ -234,10 +252,9 @@ def logprob(xhat_nd, mu_pd, sigma_pd, layout=MGP_OUT_LOGP_NP, B=None, HW=None, e
     if ws is None and m == MGP_MATH_TC_ISO and lib.mgp_logprob_ws_is_prototype_only(int(layout), P, D, m):
         cache_key = (mu.data_ptr(), mu._version, sg.data_ptr(), sg._version, P, D, float(eps), float(eps_log),
                      str(x.device), _stream())
-        hit = _PROTO_OPERANDS.get(cache_key)
-        if hit is not None and hit[0].numel() >= nbytes:
-            ws, m = hit[0], MGP_MATH_TC_ISO_REUSE
-            _PROTO_OPERANDS.move_to_end(cache_key)
+        ws = _cached_operands(_PROTO_OPERANDS, cache_key, nbytes)
+        if ws is not None:
+            m = MGP_MATH_TC_ISO_REUSE
     if ws is None:
         ws = torch.empty((max(16, nbytes),), device=x.device, dtype=torch.uint8)
     elif ws.numel() < nbytes:
@@ -245,15 +262,9 @@ def logprob(xhat_nd, mu_pd, sigma_pd, layout=MGP_OUT_LOGP_NP, B=None, HW=None, e
     check(lib.mgp_logprob_fwd(x.data_ptr(), mu.data_ptr(), sg.data_ptr(), float(eps), float(eps_log), out.data_ptr(),
                               int(layout), B_, HW_, P, D, m, ws.data_ptr(), nbytes, _stream()), "mgp_logprob_fwd")
     if cache_key is not None and m == MGP_MATH_TC_ISO:
-        # (the entry keeps mu / sigma alive, so their addresses cannot be recycled under the key)
-        _PROTO_OPERANDS[cache_key] = (ws, mu, sg)
-        while len(_PROTO_OPERANDS) > 2:
-            _PROTO_OPERANDS.popitem(last=False)
+        _keep_operands(_PROTO_OPERANDS, cache_key, ws, mu, sg)
     _count(1 if m in (MGP_MATH_TC_REUSE, MGP_MATH_TC_ISO_REUSE) else (3 if nbytes > (P * D + P) * 4 else 2))
     return (out, ws) if return_ws else out
-
-
-_DENSITY_OPERANDS = collections.OrderedDict()   # as _PROTO_OPERANDS, for log_density's tensor-core workspace
 
 
 @_on_device
@@ -287,10 +298,9 @@ def log_density(xhat_nd, mu_pd, sigma_pd, weight_cp, B, HW, C, K, math="auto", w
     if m == MGP_MATH_TC_ISO and D in (64, 128) and K <= 64:
         # the tensor-core path keeps only prototype-side operands in its workspace (plus log pi, rebuilt every call)
         cache_key = (mu.data_ptr(), mu._version, sg.data_ptr(), sg._version, P, D, str(x.device), _stream())
-        hit = _DENSITY_OPERANDS.get(cache_key)
-        if hit is not None and hit[0].numel() >= nbytes:
-            ws, m = hit[0], MGP_MATH_TC_ISO_REUSE
-            _DENSITY_OPERANDS.move_to_end(cache_key)
+        ws = _cached_operands(_DENSITY_OPERANDS, cache_key, nbytes)
+        if ws is not None:
+            m = MGP_MATH_TC_ISO_REUSE
     if ws is None:
         ws = torch.empty((max(16, nbytes),), device=x.device, dtype=torch.uint8)
     out_c = torch.empty((B, C, HW), device=x.device, dtype=torch.float32)
@@ -298,9 +308,7 @@ def log_density(xhat_nd, mu_pd, sigma_pd, weight_cp, B, HW, C, K, math="auto", w
     check(lib.mgp_log_density(x.data_ptr(), mu.data_ptr(), sg.data_ptr(), w.data_ptr(), out_c.data_ptr(), _p(out_a),
                               B, HW, C, K, D, m, ws.data_ptr(), nbytes, _stream()), "mgp_log_density")
     if cache_key is not None and m == MGP_MATH_TC_ISO:
-        _DENSITY_OPERANDS[cache_key] = (ws, mu, sg)      # (keeps mu / sigma alive: their addresses stay theirs)
-        while len(_DENSITY_OPERANDS) > 2:
-            _DENSITY_OPERANDS.popitem(last=False)
+        _keep_operands(_DENSITY_OPERANDS, cache_key, ws, mu, sg)
     _count(2 if m == MGP_MATH_TC_ISO_REUSE else 3)
     return out_c, out_a
 
