@@ -503,14 +503,20 @@ logprob_tc_kernel(const __grid_constant__ CUtensorMap map_xh, const __grid_const
 //   warp 9   TMA producer of the x tile: one NI-row box per K block and hi / lo half, each K block with its own
 //            full / empty barrier pair, so the next image's first K block loads while the current image's last
 //            prototype tile still multiplies its second one
-//   warp 8   TMA producer of the prototype K blocks (128 rows) through an S-stage ring
+//   warp 8   TMA producer of the prototype half tiles through an S-stage ring: a stage is one warpgroup's 64 rows of
+//            one K block (hi and lo, 16 KiB through a 64-row box), loaded in the order the warpgroups consume them --
+//            per prototype tile warpgroup 0's K blocks, then warpgroup 1's -- and released by the 4 warps that read it
 //   warps 0-7  warpgroup g multiplies prototype rows [64 g, 64 g + 64) of the tile with the whole image: per k16
 //            step one m64nNIk16 MMA per pass (hi*hi, lo*hi, hi*lo), one commit group per K block, the previous K
-//            block's group retired (and its stage released) while the current one runs.  The epilogue reads the
-//            fragments in place: a thread holds 2 prototype rows x NI / 4 columns; it keeps the running (max, first
-//            column) of each row, a quad of lanes merges its four by two shuffles, and lane 0 of the quad writes the
-//            packed result with a plain 64-bit store -- every (image, prototype) pair has exactly one writer, so
-//            `best` needs no zeroing and no atomics.
+//            block's group retired (and its stage released) while the current one runs.  The warpgroups take turns
+//            issuing (ping-pong, ordered by two named barriers): warpgroup 0 issues tile j while warpgroup 1 runs the
+//            epilogue of tile j - 1, then warpgroup 1 issues tile j while warpgroup 0 runs the epilogue of tile j, so
+//            the tensor cores always have the other warpgroup's MMAs queued behind the ones that finish.  The epilogue
+//            reads the fragments in place: a thread holds 2 prototype rows x NI / 4 columns; it keeps the running (max,
+//            first column) of each row, a quad of lanes merges its four by two shuffles, and lane 0 of the quad writes
+//            the packed result with a plain 64-bit store -- every (image, prototype) pair has exactly one writer, so
+//            `best` needs no zeroing and no atomics.  Turns change nothing a result depends on: each accumulator
+//            element receives the same MMAs in the same order as without them.
 // HW_MIN: the smallest HW this width serves; 8-column blocks below it need no mask.
 template <int NI, int HW_MIN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
@@ -520,6 +526,8 @@ logprob_top1_wide_kernel(const __grid_constant__ CUtensorMap map_xh, const __gri
     static_assert(NI % 8 == 0 && NI >= 32 && NI <= 256 && HW_MIN <= NI, "wgmma N");
     constexpr int R = NI / 2;                                     // accumulator registers per thread
     constexpr uint32_t XSUB = (uint32_t)NI * KB * 2;              // one [NI x 64] fp16 block of the x tile
+    constexpr uint32_t HSUB = 64u * KB * 2;                       // one warpgroup's [64 x 64] fp16 half of a K block
+    constexpr int SMAX = 8;                                       // prototype stages at most (barrier slots)
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;                 // SWIZZLE_128B tiles need 1024 B alignment
@@ -532,25 +540,28 @@ logprob_top1_wide_kernel(const __grid_constant__ CUtensorMap map_xh, const __gri
     const int nkb = prm.D / KB;                                   // 1 or 2 K blocks, the [x] / [-2 w mu] half only
     const int kcol0 = prm.D;
 
-    // carve-up: nbuf x tiles (hi blocks then lo blocks) | S prototype stages | barriers | |x|^2 of two images
+    // carve-up: nbuf x tiles (hi blocks then lo blocks) | S prototype half-tile stages (hi, lo) | barriers | |x|^2 of
+    // two images per warpgroup
     const uint32_t x_bytes = (uint32_t)(2 * nkb) * XSUB;
-    const uint32_t tile_budget = prm.smem_bytes - 1024u - 4096u;
-    const int nbuf = (2 * x_bytes + 4 * 2 * SUB_BYTES <= tile_budget) ? 2 : 1;   // double-buffer x when 4 stages still fit
-    int S = (int)((tile_budget - nbuf * x_bytes) / (2 * SUB_BYTES));
-    if (S > 6) S = 6;
+    const uint32_t misc_bytes = 256u + 2u * 2u * 256u * 4u;
+    const uint32_t tile_budget = prm.smem_bytes - 1024u - misc_bytes;
+    const int nbuf = (2 * x_bytes + 8 * 2 * HSUB <= tile_budget) ? 2 : 1;   // double-buffer x when 8 stages still fit
+    int S = (int)((tile_budget - nbuf * x_bytes) / (2 * HSUB));
+    if (S > SMAX) S = SMAX;
     const uint32_t x_base = base;
     const uint32_t st_base = x_base + nbuf * x_bytes;
-    const uint32_t misc = st_base + (uint32_t)S * 2 * SUB_BYTES;
-    const uint32_t bar0 = misc;                                   // full[6] empty[6] xfull[2][2] xempty[2][2]
+    const uint32_t misc = st_base + (uint32_t)S * 2 * HSUB;
+    const uint32_t bar0 = misc;                                   // full[8] empty[8] xfull[2][2] xempty[2][2]
     auto FULL = [&](int i) { return bar0 + 8u * i; };
-    auto EMPTY = [&](int i) { return bar0 + 8u * (6 + i); };
-    auto XFULL = [&](int b, int kb) { return bar0 + 8u * (12 + 2 * b + kb); };
-    auto XEMPTY = [&](int b, int kb) { return bar0 + 8u * (16 + 2 * b + kb); };
-    float* s_sn = reinterpret_cast<float*>(base_ptr + (misc - base) + 256);   // [2][256]
+    auto EMPTY = [&](int i) { return bar0 + 8u * (SMAX + i); };
+    auto XFULL = [&](int b, int kb) { return bar0 + 8u * (2 * SMAX + 2 * b + kb); };
+    auto XEMPTY = [&](int b, int kb) { return bar0 + 8u * (2 * SMAX + 4 + 2 * b + kb); };
+    float* s_sn = reinterpret_cast<float*>(base_ptr + (misc - base) + 256);   // [2 warpgroups][2 images][256]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
-        for (int i = 0; i < 6; ++i) { mbar_init(FULL(i), 1); mbar_init(EMPTY(i), 8); }   // empty: one arrive per consumer warp
+        // prototype empty: one arrive per warp of the warpgroup that read the stage; x empty: per consumer warp
+        for (int i = 0; i < SMAX; ++i) { mbar_init(FULL(i), 1); mbar_init(EMPTY(i), 4); }
         for (int b = 0; b < 2; ++b)
             for (int kb = 0; kb < 2; ++kb) { mbar_init(XFULL(b, kb), 1); mbar_init(XEMPTY(b, kb), 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -579,42 +590,56 @@ logprob_top1_wide_kernel(const __grid_constant__ CUtensorMap map_xh, const __gri
         }
     } else if (warp == 8) {
         // =========================== prototype TMA producer ===========================
+        // stage order per prototype tile: warpgroup 0's K blocks, then warpgroup 1's
         if (lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
             for (int nt = team; nt < B; nt += n_teams)
                 for (int pt = k0; pt < n_ptiles; pt += TS)
-                    for (int kb = 0; kb < nkb; ++kb) {
-                        mbar_wait(EMPTY(stage), phase ^ 1u);
-                        if (prm.debug & 16) {
-                            mbar_arrive(FULL(stage));
-                        } else {
-                            mbar_expect_tx(FULL(stage), 2 * SUB_BYTES);
-                            const uint32_t dst = st_base + (uint32_t)stage * 2 * SUB_BYTES;
-                            tma_load_2d(dst, &map_ph, kcol0 + kb * KB, pt * PT, FULL(stage));
-                            tma_load_2d(dst + SUB_BYTES, &map_pl, kcol0 + kb * KB, pt * PT, FULL(stage));
+                    for (int h = 0; h < 2; ++h)
+                        for (int kb = 0; kb < nkb; ++kb) {
+                            const int r0 = pt * PT + 64 * h;
+                            mbar_wait(EMPTY(stage), phase ^ 1u);
+                            if ((prm.debug & 16) || r0 >= prm.P) {
+                                // no load: switched off, or no prototype row in this half (its results are not stored)
+                                mbar_arrive(FULL(stage));
+                            } else {
+                                mbar_expect_tx(FULL(stage), 2 * HSUB);
+                                const uint32_t dst = st_base + (uint32_t)stage * 2 * HSUB;
+                                tma_load_2d(dst, &map_ph, kcol0 + kb * KB, r0, FULL(stage));
+                                tma_load_2d(dst + HSUB, &map_pl, kcol0 + kb * KB, r0, FULL(stage));
+                            }
+                            if (++stage == S) { stage = 0; phase ^= 1u; }
                         }
-                        if (++stage == S) { stage = 0; phase ^= 1u; }
-                    }
         }
     } else {
         // =========================== consumers: MMA + epilogue ===========================
-        const int wg = warp >> 2, wq = warp & 3, q = lane & 3;
+        const int wg = warp >> 2, wq = warp & 3, q = lane & 3, u = threadIdx.x & 127;
         const int prow = wg * 64 + 16 * wq + (lane >> 2);         // this thread's prototype rows: prow and prow + 8
         unsigned long long* best = reinterpret_cast<unsigned long long*>(prm.out);
-        int stage = 0, c = 0;
+        // turns: named barrier 4 + g = "warpgroup g may issue its MMAs of the next tile" (one warpgroup arrives, the
+        // other waits, 256 threads; 2 + g syncs warpgroup g alone); warpgroup 0 takes the first turn without waiting,
+        // and warpgroup 1 hands a turn back only when another tile follows, so every arrive has its wait
+        auto wait_turn = [&]() { if (wg) named_bar_sync<5, 256>(); else named_bar_sync<4, 256>(); };
+        auto give_turn = [&]() { if (wg) named_bar_arrive<4, 256>(); else named_bar_arrive<5, 256>(); };
+        // ring position: this warpgroup's stages of a tile follow nkb stages of warpgroup 0 (for warpgroup 1) and are
+        // followed by nkb of warpgroup 1 (for warpgroup 0); nkb <= 2 < S
+        int stage = wg * nkb, c = 0;
         uint32_t phase = 0;
+        auto advance = [&](int n) { stage += n; if (stage >= S) { stage -= S; phase ^= 1u; } };
+        bool first = true;
         for (int nt = team; nt < B; nt += n_teams, ++c) {
             const int buf = c % nbuf;
             const uint32_t xpar = (uint32_t)((c / nbuf) & 1);
             const uint32_t xb = x_base + (uint32_t)buf * x_bytes;
-            // |x|^2 of this image, double-buffered by image: the readers of buffer c & 1 (image c - 2) all passed
-            // the previous image's barrier
-            float* sn = s_sn + (c & 1) * 256;
-            for (int i = threadIdx.x; i < NI; i += 256) sn[i] = (i < HW) ? prm.sn[(size_t)nt * HW + i] : 0.f;
-            asm volatile("bar.sync 1, 256;" ::: "memory");
+            // |x|^2 of this image, a copy per warpgroup so that neither waits for the other, double-buffered by image:
+            // the readers of buffer c & 1 (image c - 2) are this warpgroup's threads, all past the previous image's barrier
+            float* sn = s_sn + wg * 512 + (c & 1) * 256;
+            for (int i = u; i < NI; i += 128) sn[i] = (i < HW) ? prm.sn[(size_t)nt * HW + i] : 0.f;
+            if (wg) named_bar_sync<3, 128>(); else named_bar_sync<2, 128>();
             for (int pt = k0; pt < n_ptiles; pt += TS) {
                 const bool last = pt + TS >= n_ptiles;            // last prototype tile of this image: release x
+                const bool more = !last || nt + n_teams < B;      // another tile follows in this CTA
                 const int p0 = pt * PT + prow, p1 = p0 + 8;
                 const float c0a = p0 < prm.P ? __ldg(prm.e0 + p0) : 0.f, c0b = p1 < prm.P ? __ldg(prm.e0 + p1) : 0.f;
                 const float c1a = p0 < prm.P ? __ldg(prm.e1 + p0) : 0.f, c1b = p1 < prm.P ? __ldg(prm.e1 + p1) : 0.f;
@@ -622,13 +647,15 @@ logprob_top1_wide_kernel(const __grid_constant__ CUtensorMap map_xh, const __gri
                 float acc[R];
 #pragma unroll
                 for (int j = 0; j < R; ++j) acc[j] = 0.f;
+                if (wg == 1 || !first) wait_turn();               // the other warpgroup has issued its MMAs
+                first = false;
                 int prev = 0;
                 for (int kb = 0; kb < nkb; ++kb) {
                     mbar_wait(XFULL(buf, kb), xpar);
                     mbar_wait(FULL(stage), phase);
                     if (!(prm.debug & 4)) {
-                        const uint32_t ph = st_base + (uint32_t)stage * 2 * SUB_BYTES + (uint32_t)wg * 64u * 128u;
-                        const uint32_t pl = ph + SUB_BYTES;
+                        const uint32_t ph = st_base + (uint32_t)stage * 2 * HSUB;
+                        const uint32_t pl = ph + HSUB;
                         const uint32_t xh = xb + (uint32_t)kb * XSUB, xl = xb + (uint32_t)(nkb + kb) * XSUB;
                         wg_fence();
 #pragma unroll
@@ -642,6 +669,8 @@ logprob_top1_wide_kernel(const __grid_constant__ CUtensorMap map_xh, const __gri
                         }
                         wg_commit();
                     }
+                    // every MMA of this tile is issued: the other warpgroup's turn (its MMAs queue behind these)
+                    if (kb == nkb - 1 && (wg == 0 || more)) give_turn();
                     if (kb > 0) {                                 // K block kb - 1 has retired: release what it read
                         wg_wait<1>();
                         __syncwarp();
@@ -651,8 +680,9 @@ logprob_top1_wide_kernel(const __grid_constant__ CUtensorMap map_xh, const __gri
                         }
                     }
                     prev = stage;
-                    if (++stage == S) { stage = 0; phase ^= 1u; }
+                    advance(1);
                 }
+                advance(nkb);                                     // past the other warpgroup's stages of this tile
                 wg_wait<0>();
                 wg_fence_operands(acc);
                 __syncwarp();
@@ -881,10 +911,12 @@ int mgp_logprob_tc_launch(const float* xhat, const float* mu, const float* sigma
     prm.smem_bytes = (uint32_t)smem;
 
     if (top1_wide) {
-        // the x map's box is the whole image tile (NI rows, NI = HW rounded up to an instantiated width)
+        // the x map's box is the whole image tile (NI rows, NI = HW rounded up to an instantiated width); the prototype
+        // maps' box is one warpgroup's 64 rows (the kernel's ring stages are half tiles)
         const int ni = HW <= 32 ? 32 : HW <= 56 ? 56 : HW <= 64 ? 64 : HW <= 128 ? 128 : HW <= 200 ? 200 : 256;
-        CUtensorMap wxh, wxl;
-        if (!make_map_f16(&wxh, ah, (uint64_t)N, 2 * D, (uint32_t)ni) || !make_map_f16(&wxl, al, (uint64_t)N, 2 * D, (uint32_t)ni))
+        CUtensorMap wxh, wxl, wph, wpl;
+        if (!make_map_f16(&wxh, ah, (uint64_t)N, 2 * D, (uint32_t)ni) || !make_map_f16(&wxl, al, (uint64_t)N, 2 * D, (uint32_t)ni) ||
+            !make_map_f16(&wph, bh, (uint64_t)P, 2 * D, 64) || !make_map_f16(&wpl, bl, (uint64_t)P, 2 * D, 64))
             return MGP_ERR_UNSUPPORTED;
         TcParams pw = prm;
         pw.iso_elsewhere = iso_known ? 0 : 1;
@@ -893,7 +925,7 @@ int mgp_logprob_tc_launch(const float* xhat, const float* mu, const float* sigma
     do {                                                                                                           \
         MGP_CUDA(cudaFuncSetAttribute(logprob_top1_wide_kernel<NI, LO>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
                                       (int)smem));                                                                 \
-        logprob_top1_wide_kernel<NI, LO><<<grid_w, TC_THREADS, smem, st>>>(wxh, wxl, mph, mpl, pw);               \
+        logprob_top1_wide_kernel<NI, LO><<<grid_w, TC_THREADS, smem, st>>>(wxh, wxl, wph, wpl, pw);               \
     } while (0)
         switch (ni) {
             case 32: MGP_TOP1_WIDE(32, 32); break;

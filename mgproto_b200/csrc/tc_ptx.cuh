@@ -59,6 +59,18 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         }
     }
 }
+// Named barriers (bar.sync / bar.arrive, ids 1..15; 0 is __syncthreads): THREADS counts every participant, waiting
+// or arriving, and is a multiple of 32.  A warpgroup that arrives does not wait, so a pair of them orders two
+// warpgroups without making the signalling one block.  The id is an immediate, so ptxas reserves only the barriers a
+// kernel names.
+template <int ID, int THREADS>
+__device__ __forceinline__ void named_bar_sync() {
+    asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(THREADS) : "memory");
+}
+template <int ID, int THREADS>
+__device__ __forceinline__ void named_bar_arrive() {
+    asm volatile("bar.arrive %0, %1;" ::"n"(ID), "n"(THREADS) : "memory");
+}
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
