@@ -207,6 +207,31 @@ int mgp_head_bwd_x(const float* grad_logits, const float* logits, const float* v
                    const float* sigma, void* ws, size_t ws_bytes, void* g_x, int x_fmt, int B,
                    int HW, int C, int K, int D, int T, void* stream);
 
+/* ---- long feature maps: the head at 1 <= HW <= 4096 -----------------------------------------
+ * ref: model.py:188-206 (global_max_pooling_gmm_topT: torch.topk over h*w of any size), :214-222, :254.
+ * The entry points above refuse HW > 1024 (10-bit patch keys, [HW]-sized shared-memory tiles); these take any
+ * HW <= 4096 (2048-px inputs at stride 32, 1024-px inputs with the x2 add-on upsample, model.py:138), with
+ * T <= min(32, HW) and K <= 64, and compute the same outputs.  HW > 4096 returns MGP_ERR_UNSUPPORTED before any
+ * launch.  Shared memory per block does not depend on HW.
+ * mgp_head_select_long: as mgp_head_select (logp_bphw [B,P,HW]; gt may be NULL). */
+int mgp_head_select_long(const float* logp_bphw, const float* weight_cp, const int64_t* gt,
+                         float* logits, float* vals, int32_t* idx, int B, int HW, int C, int K,
+                         int T, void* stream);
+/* As mgp_head_select_top1 (ref model.py:218-221): `best` [B,P] from mgp_logprob_fwd(MGP_OUT_TOP1_BP), the own
+ * class's exact fp32 log p evaluated in patch slices; gt = -1 for every image gives the level-0 head. */
+int mgp_head_select_top1_long(const uint64_t* best, const float* xhat_nd, const float* mu,
+                              const float* sigma, const float* weight_cp, const int64_t* gt,
+                              float* logits, float* vals, int32_t* idx, int B, int HW, int C,
+                              int K, int D, int T, void* stream);
+/* As mgp_head_bwd_x (ref model.py:210-222 backward), for the outputs of the two calls above; deterministic and
+ * atomics-free like it.  Also needs P = C*K < 2^20.  ws: mgp_head_bwd_long_ws_bytes(B, HW, P, D) bytes. */
+size_t mgp_head_bwd_long_ws_bytes(int B, int HW, int P, int D);
+int mgp_head_bwd_long_x(const float* grad_logits, const float* logits, const float* vals,
+                        const int32_t* idx, const float* weight_cp, const int64_t* gt,
+                        const float* xhat_nd, const float* inv_norm, const float* mu,
+                        const float* sigma, void* ws, size_t ws_bytes, void* g_x, int x_fmt,
+                        int B, int HW, int C, int K, int D, int T, void* stream);
+
 /* ref: model.py:188-206 (global_max_pooling_gmm_topT) as a stand-alone call on PROBABILITIES sims [B,P,HW]:
  * vals [B,P,T] = the T largest over HW, descending; idx [B,P,T] their patch indices; feats [B,P,D,T] (optional, NULL
  * to skip; 4*B*P*D*T bytes) = x_nchw[b, :, idx[b,p,t]] -- the reference's max_feat, [B,C,K,D,T] once viewed. */

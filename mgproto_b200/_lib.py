@@ -41,6 +41,10 @@ SIGNATURES = {
     "mgp_head_bwd_ws_bytes": (_sz, [_i, _i, _i, _i]),
     "mgp_head_bwd": (_i, [_vp] * 11 + [_sz, _vp] + [_i] * 6 + [_vp]),
     "mgp_head_bwd_x": (_i, [_vp] * 11 + [_sz, _vp] + [_i] * 7 + [_vp]),
+    "mgp_head_select_long": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "mgp_head_select_top1_long": (_i, [_vp] * 9 + [_i] * 6 + [_vp]),
+    "mgp_head_bwd_long_ws_bytes": (_sz, [_i, _i, _i, _i]),
+    "mgp_head_bwd_long_x": (_i, [_vp] * 11 + [_sz, _vp] + [_i] * 7 + [_vp]),
     "mgp_mined_gather": (_i, [_vp] * 5 + [_i] * 8 + [_vp]),
     "mgp_bank_enqueue": (_i, [_vp] * 7 + [_i] * 3 + [_vp] * 4 + [_i] * 5 + [_vp]),
     "mgp_bank_enqueue_plan_ints": (_sz, [_i, _i, _i]),

@@ -5,141 +5,9 @@
 #include "mgp_common.cuh"
 #include <type_traits>
 
+#include "head_topt.cuh"
+
 namespace {
-
-// One warp selects the T largest of NR [HW] rows at once (descending, ties -> smaller index).
-// Each lane keeps R = ceil(HW/32) keys per row in registers; per level: warp REDUX.max on the lanes'
-// local maxima, REDUX.min on the index among equal maxima, winner removed from its lane.  The NR rows
-// are independent dependency chains, interleaved to hide the REDUX latency.
-template <int R, int NR>
-__device__ __forceinline__ void warp_topT(const float* const (&rows)[NR], int rs, int HW, int T, int lane,
-                                          float (&out_v)[NR], int (&out_i)[NR]) {
-    unsigned key[NR][R];
-#pragma unroll
-    for (int i = 0; i < NR; ++i) {
-#pragma unroll
-        for (int r = 0; r < R; ++r) {
-            const int j = lane + 32 * r;
-            key[i][r] = (j < HW) ? f2key(rows[i][(size_t)j * rs]) : 0u;  // 0 sorts below every real float (incl. -inf)
-        }
-        out_v[i] = 0.f;
-        out_i[i] = 0;
-    }
-    for (int t = 0; t < T; ++t) {
-#pragma unroll
-        for (int i = 0; i < NR; ++i) {
-            unsigned lm = key[i][0];
-#pragma unroll
-            for (int r = 1; r < R; ++r) lm = max(lm, key[i][r]);
-            int li = 0x7fffffff;
-#pragma unroll
-            for (int r = R - 1; r >= 0; --r)
-                if (key[i][r] == lm) li = lane + 32 * r;
-            const unsigned best = __reduce_max_sync(0xffffffffu, lm);
-            const int bi = __reduce_min_sync(0xffffffffu, (lm == best) ? li : 0x7fffffff);
-#pragma unroll
-            for (int r = 0; r < R; ++r)
-                if (bi == lane + 32 * r) key[i][r] = 0u;
-            if (lane == t) {
-                out_v[i] = key2f(best);
-                out_i[i] = bi;
-            }
-        }
-    }
-}
-
-// Faster variant for R <= 8 (HW <= 256): every lane first sorts its R keys (descending, compile-time
-// compare-exchange network), so a level costs one REDUX.max over the lanes' heads, a ballot to find the
-// owner (lowest lane among equal heads) and a predicated pop of the owner's list -- ~15 instructions instead
-// of ~45.  Indices are recovered at the end from the owner's unsorted copy: lane t fetches the owner's R
-// original keys by shuffle and takes the position of its value; equal values picked twice from one lane
-// are disambiguated by their rank among earlier identical picks (MATCH.ANY).
-template <int R, int NR>
-__device__ __forceinline__ void warp_topT_sorted(const float* const (&rows)[NR], int rs, int HW, int T, int lane,
-                                                 float (&out_v)[NR], int (&out_i)[NR]) {
-    unsigned orig[NR][R], key[NR][R];
-#pragma unroll
-    for (int i = 0; i < NR; ++i) {
-#pragma unroll
-        for (int r = 0; r < R; ++r) {
-            const int j = lane + 32 * r;
-            orig[i][r] = (j < HW) ? f2key(rows[i][(size_t)j * rs]) : 0u;
-            key[i][r] = orig[i][r];
-        }
-#pragma unroll
-        for (int a = 1; a < R; ++a)
-#pragma unroll
-            for (int b = a; b >= 1; --b) {
-                const unsigned hi = max(key[i][b - 1], key[i][b]), lo = min(key[i][b - 1], key[i][b]);
-                key[i][b - 1] = hi;
-                key[i][b] = lo;
-            }
-    }
-    unsigned my_key[NR];
-    int my_owner[NR];
-#pragma unroll
-    for (int i = 0; i < NR; ++i) { my_key[i] = 0u; my_owner[i] = 0; }
-    for (int t = 0; t < T; ++t) {
-#pragma unroll
-        for (int i = 0; i < NR; ++i) {
-            const unsigned best = __reduce_max_sync(0xffffffffu, key[i][0]);
-            const unsigned m = __ballot_sync(0xffffffffu, key[i][0] == best);
-            const int owner = __ffs(m) - 1;
-            if (lane == owner) {
-#pragma unroll
-                for (int r = 0; r + 1 < R; ++r) key[i][r] = key[i][r + 1];
-                key[i][R - 1] = 0u;
-            }
-            if (lane == t) { my_key[i] = best; my_owner[i] = owner; }
-        }
-    }
-#pragma unroll
-    for (int i = 0; i < NR; ++i) {
-        // rank of this pick among earlier picks of the same (value, lane)
-        const unsigned long long tag = ((unsigned long long)my_key[i] << 8) | (unsigned)my_owner[i];
-        const unsigned same = __match_any_sync(0xffffffffu, (lane < T) ? tag : (0xffffffffffffff00ull | (unsigned)lane));
-        int skip = __popc(same & ((1u << lane) - 1u));
-        int rr = 0;
-#pragma unroll
-        for (int r = 0; r < R; ++r) {
-            const unsigned o = __shfl_sync(0xffffffffu, orig[i][r], my_owner[i]);
-            const bool hit = (o == my_key[i]);
-            if (hit && skip == 0) rr = r;
-            if (hit) --skip;
-        }
-        out_v[i] = key2f(my_key[i]);
-        out_i[i] = my_owner[i] + 32 * rr;
-    }
-}
-
-// Level 0 only (max and arg-max, ties -> smaller index) of NR rows: with labels the reference overwrites
-// levels >= 1 of every wrong-class prototype with level 0 (model.py:218-221), so only the K rows of the
-// image's own class need the full top-T.  ~40 instructions per row instead of ~540: the kernel becomes a
-// streaming read of log p.
-template <int R, int NR>
-__device__ __forceinline__ void warp_top1(const float* const (&rows)[NR], int rs, int HW, int lane,
-                                          float (&out_v)[NR], int (&out_i)[NR]) {
-    float x[NR][R];
-#pragma unroll
-    for (int i = 0; i < NR; ++i)
-#pragma unroll
-        for (int r = 0; r < R; ++r) {
-            const int j = lane + 32 * r;
-            x[i][r] = (j < HW) ? rows[i][(size_t)j * rs] : -INFINITY;
-        }
-#pragma unroll
-    for (int i = 0; i < NR; ++i) {
-        float mv = x[i][0];
-        int mr = 0;
-#pragma unroll
-        for (int r = 1; r < R; ++r)
-            if (x[i][r] > mv) { mv = x[i][r]; mr = r; }
-        const unsigned key = (lane < HW) ? f2key(mv) : 0u;
-        const unsigned best = __reduce_max_sync(0xffffffffu, key);
-        out_i[i] = __reduce_min_sync(0xffffffffu, (key == best) ? lane + 32 * mr : 0x7fffffff);
-        out_v[i] = key2f(best);
-    }
-}
 
 // FROM_NP = false: logp is [B,P,HW] (one contiguous row per (image, prototype)).
 // FROM_NP = true : logp is [N,P] (the compute_log_prob / tensor-core layout): the CTA first stages the
@@ -431,360 +299,19 @@ __global__ void proto_weight_kernel(const float* __restrict__ mu, const float* _
     }
 }
 
-constexpr int LCAP = 2304;   // entries per drain (>= P + K(T-1) of the labelled cfg: one drain per image)
+}  // namespace
 
-// grid (B, D/DC), DC = 32 VEC (VEC = 4 floats per lane when D is a multiple of 128: ONE CTA per image at D = 128, so the
-// list is built and sorted once; VEC = 2 otherwise): CTA (b, j) produces dims [DC j, DC j + DC) of image b's rows of
-// g_xhat (zeroed by the caller).  Entries with gradient are compacted in a fixed order, stably counting-sorted by patch row, then each
-// warp walks one eighth of the sorted list with lanes owning two dims each (see the walk below) and adds every
-// finished row straight into global memory (a row has exactly one writer per drain): balanced however the mined
-// patches cluster, no atomics, fixed summation order, 48 KB of shared memory -> 4 CTAs per SM.
-template <int VEC> struct LaneVec { float v[VEC]; };
-template <int VEC>
-__device__ __forceinline__ LaneVec<VEC> lv_ldg(const float* p) {
-    LaneVec<VEC> r;
-    if constexpr (VEC == 4) { const float4 t = __ldg(reinterpret_cast<const float4*>(p)); r.v[0] = t.x; r.v[1] = t.y; r.v[2] = t.z; r.v[3] = t.w; }
-    else { const float2 t = __ldg(reinterpret_cast<const float2*>(p)); r.v[0] = t.x; r.v[1] = t.y; }
-    return r;
-}
-template <int VEC>
-__device__ __forceinline__ LaneVec<VEC> lv_ldcg(const float* p) {
-    LaneVec<VEC> r;
-    if constexpr (VEC == 4) { const float4 t = __ldcg(reinterpret_cast<const float4*>(p)); r.v[0] = t.x; r.v[1] = t.y; r.v[2] = t.z; r.v[3] = t.w; }
-    else { const float2 t = __ldcg(reinterpret_cast<const float2*>(p)); r.v[0] = t.x; r.v[1] = t.y; }
-    return r;
-}
-template <int VEC>
-__device__ __forceinline__ LaneVec<VEC> lv_ld(const float* p) {
-    LaneVec<VEC> r;
-    if constexpr (VEC == 4) { const float4 t = *reinterpret_cast<const float4*>(p); r.v[0] = t.x; r.v[1] = t.y; r.v[2] = t.z; r.v[3] = t.w; }
-    else { const float2 t = *reinterpret_cast<const float2*>(p); r.v[0] = t.x; r.v[1] = t.y; }
-    return r;
-}
-template <int VEC>
-__device__ __forceinline__ void lv_st(float* p, const LaneVec<VEC>& r) {
-    if constexpr (VEC == 4) *reinterpret_cast<float4*>(p) = make_float4(r.v[0], r.v[1], r.v[2], r.v[3]);
-    else *reinterpret_cast<float2*>(p) = make_float2(r.v[0], r.v[1]);
-}
-template <int VEC>
-__device__ __forceinline__ LaneVec<VEC> lv_zero() {
-    LaneVec<VEC> r;
-#pragma unroll
-    for (int i = 0; i < VEC; ++i) r.v[i] = 0.f;
-    return r;
-}
+#include "head_bwd.cuh"
+
+namespace {
 
 template <int VEC>
-__global__ void __launch_bounds__(256, VEC == 4 ? 2 : 4)
-head_bwd_kernel(const float* __restrict__ gl, const float* __restrict__ logits, const float* __restrict__ vals,
-                const int32_t* __restrict__ idx, const float* __restrict__ weight, const int64_t* __restrict__ gt,
-                const float* __restrict__ xhat, const float* __restrict__ w, const float* __restrict__ wm,
-                const float* __restrict__ wsc, const int* __restrict__ noniso, float* __restrict__ g_xhat, int HW,
-                int C, int K, int D, int T) {
-    constexpr int DC = 32 * VEC;
-    using LV = LaneVec<VEC>;
-    extern __shared__ float smem[];
-    const bool aniso = (*noniso != 0);
-    unsigned* lkey = reinterpret_cast<unsigned*>(smem);     // [LCAP] p*1024 + n
-    float* lval = reinterpret_cast<float*>(lkey + LCAP);    // [LCAP]
-    unsigned* skey = reinterpret_cast<unsigned*>(lval + LCAP);                // [LCAP] sorted by row
-    float* sval = reinterpret_cast<float*>(skey + LCAP);    // [LCAP]
-    int* bins = reinterpret_cast<int*>(sval + LCAP);        // [8][HW] per-warp row histograms / start offsets
-    float* Qs = reinterpret_cast<float*>(bins + 8 * HW);    // [C]  sum_t gl/exp(logit)      (wrong-class fold)
-    float* qg = Qs + C;                                     // [T]  gl/exp(logit) of the GT class
-    __shared__ int wcount[8];
-    __shared__ int lcount;
-    __shared__ __align__(16) float part[16 * DC];           // boundary runs of the warps' list ranges (s1 vectors)
-    __shared__ float part2[16];                             // ... their scalar sum_e a_e w_p (isotropic sigma)
-    __shared__ int prow[16];
-    __shared__ int mrow[16], mcount;                        // boundary runs merged by row
-
-    const int b = blockIdx.x;
-    const int d0 = blockIdx.y * DC;
-    const int dc = min(DC, D - d0);
-    const int P = C * K;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const bool has_gt = (gt != nullptr);
-    const long long g = has_gt ? (long long)gt[b] : -1;
-
-    if (has_gt) {
-        if (C * T <= 2 * LCAP) {
-            // q[c][t] = gl / exp(logit) for the whole image in one coalesced pass (staged in the sorted-list
-            // area, free until the first drain), then one thread per class sums its T levels
-            float* qtmp = reinterpret_cast<float*>(skey);
-            const size_t lo = (size_t)b * C * T;
-            for (int i = threadIdx.x; i < C * T; i += 256) qtmp[i] = gl[lo + i] / expf(logits[lo + i]);
-            __syncthreads();
-            for (int c = threadIdx.x; c < C; c += 256) {
-                float q = 0.f;
-                for (int t = 0; t < T; ++t) q += qtmp[c * T + t];
-                Qs[c] = q;
-            }
-            if (g >= 0 && g < C)
-                for (int t = threadIdx.x; t < T; t += 256) qg[t] = qtmp[(int)g * T + t];
-        } else {
-            for (int c = threadIdx.x; c < C; c += 256) {
-                const size_t lo = ((size_t)b * C + c) * T;
-                float q = 0.f;
-                for (int t = 0; t < T; ++t) q += gl[lo + t] / expf(logits[lo + t]);
-                Qs[c] = q;
-            }
-            if (g >= 0 && g < C)
-                for (int t = threadIdx.x; t < T; t += 256) {
-                    const size_t lo = ((size_t)b * C + (size_t)g) * T;
-                    qg[t] = gl[lo + t] / expf(logits[lo + t]);
-                }
-        }
-    }
-    if (threadIdx.x == 0) lcount = 0;
-    __syncthreads();
-
-    // entry space: with labels only level 0 of every prototype plus levels 1..T-1 of the GT class carry
-    // gradient (wrong-class levels alias level 0, ref model.py:221); without labels all P*T entries
-    const bool gvalid = has_gt && g >= 0 && g < C;
-    const int E = has_gt ? (P + (gvalid ? K * (T - 1) : 0)) : P * T;
-    // entry e -> (coefficient a, key p*1024 + n); evaluated one iteration ahead so the gathers of the next
-    // 256 entries are in flight while the current ones are compacted
-    auto entry = [&](int e, float& a, unsigned& key) {
-        a = 0.f;
-        key = 0;
-        if (e < E) {
-            int p, t;
-            float qv;
-            if (has_gt) {
-                if (e < P) {
-                    p = e; t = 0;
-                    const int c = p / K;
-                    qv = ((long long)c == g) ? qg[0] : Qs[c];
-                } else {
-                    const int r = e - P;
-                    const int k = r / (T - 1);
-                    t = 1 + (r - k * (T - 1));
-                    p = (int)g * K + k;
-                    qv = qg[t];
-                }
-            } else {
-                p = e / T; t = e - p * T;
-                const size_t lo = ((size_t)b * C + p / K) * T + t;
-                qv = gl[lo] / expf(logits[lo]);
-            }
-            const int c = p / K;
-            const size_t vi = ((size_t)b * P + p) * T + t;
-            a = qv * __ldg(weight + (size_t)c * P + p) * vals[vi];
-            key = (unsigned)p * 1024u + (unsigned)idx[vi];
-        }
-    };
-    float a_nx;
-    unsigned key_nx;
-    entry(threadIdx.x, a_nx, key_nx);
-    for (int e0 = 0; e0 < E; e0 += 256) {
-        const float a = a_nx;
-        const unsigned key = key_nx;
-        entry(e0 + 256 + threadIdx.x, a_nx, key_nx);
-        const bool keep = (a != 0.f);
-        const unsigned bal = __ballot_sync(0xffffffffu, keep);
-        if (lane == 0) wcount[warp] = __popc(bal);
-        __syncthreads();
-        int base = lcount;
-        for (int wv = 0; wv < warp; ++wv) base += wcount[wv];
-        if (keep) {
-            const int pos = base + __popc(bal & ((1u << lane) - 1u));
-            lkey[pos] = key;
-            lval[pos] = a;
-        }
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            int tot = 0;
-            for (int wv = 0; wv < 8; ++wv) tot += wcount[wv];
-            lcount += tot;
-        }
-        __syncthreads();
-        const int cnt = lcount;
-        const bool last = (e0 + 256 >= E);
-        if (cnt + 256 > LCAP || last) {
-            // Stable counting sort of the entries by patch row (deterministic): warp w owns the w-th contiguous
-            // eighth of the list; per-warp row histograms (MATCH.ANY, leader adds) -> per-warp start offsets ->
-            // in-order scatter.  Mined patches cluster on a few dozen rows, so after the sort a lane meets long
-            // runs of one row.
-            int* whist = bins;                                  // [8][HW] per-warp histograms, then start offsets
-            for (int i = threadIdx.x; i < 8 * HW; i += 256) whist[i] = 0;
-            __syncthreads();
-            const int seg = (cnt + 7) / 8, sb = min(cnt, warp * seg), se = min(cnt, sb + seg);
-            for (int i0 = sb; i0 < se; i0 += 32) {
-                const int i = i0 + lane;
-                const int n = (i < se) ? (int)(lkey[i] & 1023u) : (0x10000 + lane);
-                const unsigned m = __match_any_sync(0xffffffffu, n);
-                if (i < se && (m & ((1u << lane) - 1u)) == 0) whist[warp * HW + n] += __popc(m);
-                __syncwarp();
-            }
-            __syncthreads();
-            // start offset of (warp, row): rows ascending, warps ascending inside a row
-            if (warp == 0) {
-                int carry = 0;
-                for (int r0 = 0; r0 < HW; r0 += 32) {
-                    const int r = r0 + lane;
-                    int tot = 0;
-                    if (r < HW)
-                        for (int wv = 0; wv < 8; ++wv) tot += whist[wv * HW + r];
-                    int x = tot;
-#pragma unroll
-                    for (int o = 1; o < 32; o <<= 1) {
-                        const int y = __shfl_up_sync(0xffffffffu, x, o);
-                        if (lane >= o) x += y;
-                    }
-                    int start = carry + x - tot;                // exclusive prefix
-                    if (r < HW)
-                        for (int wv = 0; wv < 8; ++wv) {
-                            const int c = whist[wv * HW + r];
-                            whist[wv * HW + r] = start;
-                            start += c;
-                        }
-                    carry += __shfl_sync(0xffffffffu, x, 31);
-                }
-            }
-            __syncthreads();
-            for (int i0 = sb; i0 < se; i0 += 32) {
-                const int i = i0 + lane;
-                const unsigned kk = (i < se) ? lkey[i] : 0u;
-                const int n = (i < se) ? (int)(kk & 1023u) : (0x10000 + lane);
-                const unsigned m = __match_any_sync(0xffffffffu, n);
-                if (i < se) {
-                    const int pos = whist[warp * HW + n] + __popc(m & ((1u << lane) - 1u));
-                    skey[pos] = kk;
-                    sval[pos] = lval[i];
-                }
-                __syncwarp();
-                if (i < se && (m & ((1u << lane) - 1u)) == 0) whist[warp * HW + n] += __popc(m);
-                __syncwarp();
-            }
-            __syncthreads();
-            // Walk: warp w owns the w-th eighth of the row-sorted list (balanced however the patches cluster),
-            // lanes own two dims each, so one instruction handles one entry x 64 dims and the prototype rows
-            // are read as coalesced 256-byte segments, eight in flight.  Per row n:
-            //   g[n] += sum_e a_e * wm_p  -  xhat_n * sum_e a_e * w_p
-            // (w_p is a per-prototype scalar when every sigma is isotropic).  xhat_n and the old g[n] are fetched
-            // when a run starts and used when it ends.  Runs inside a warp's range are complete rows (single
-            // writer); the first and last run of a range may continue in the neighbour's range: they are parked in
-            // `part`, merged by row in a fixed order and added afterwards -> no atomics, deterministic.
-            if (threadIdx.x < 16) prow[threadIdx.x] = -1;
-            __syncthreads();
-            const int dl = VEC * lane;
-            const bool dok2 = dl < dc;
-            const int dle = dok2 ? dl : 0;                       // lanes beyond dc shadow the first dims, never store
-            const float* xcol2 = xhat + (size_t)b * HW * D + d0 + dle;
-            float* gcol = g_xhat + (size_t)b * HW * D + d0 + dle;
-            {
-                const int wseg = (cnt + 7) / 8, wb = min(cnt, warp * wseg), we = min(cnt, wb + wseg);
-                const float* wmcol_l = wm + d0 + dle;
-                const float* wcol_l = w + d0 + dle;
-                int cur_n = -1;
-                bool first_run = true;
-                LV s1 = lv_zero<VEC>(), s2v = lv_zero<VEC>(), xpre = lv_zero<VEC>(), gpre = lv_zero<VEC>();
-                float s2 = 0.f;
-                auto flush = [&](int slot) {
-                    if (slot < 0) {
-                        LV v = gpre;
-#pragma unroll
-                        for (int i = 0; i < VEC; ++i) v.v[i] += aniso ? fmaf(-xpre.v[i], s2v.v[i], s1.v[i]) : fmaf(-xpre.v[i], s2, s1.v[i]);
-                        if (dok2) lv_st<VEC>(gcol + (size_t)cur_n * D, v);
-                    } else {
-                        LV v = s1;                                // isotropic: raw sums, xhat applied after the merge
-                        if (aniso) {
-#pragma unroll
-                            for (int i = 0; i < VEC; ++i) v.v[i] = fmaf(-xpre.v[i], s2v.v[i], v.v[i]);
-                        }
-                        if (dok2) lv_st<VEC>(part + (warp * 2 + slot) * DC + dl, v);
-                        if (lane == 0) { part2[warp * 2 + slot] = aniso ? 0.f : s2; prow[warp * 2 + slot] = cur_n; }
-                    }
-                };
-                auto walk = [&](auto aniso_tag) {
-                    constexpr bool AN = decltype(aniso_tag)::value;
-                    constexpr int PF = (VEC == 4 && !AN) ? 16 : 8;    // prototype rows in flight per lane
-                    for (int i0 = wb; i0 < we; i0 += 32) {
-                        const int i = i0 + lane;
-                        const bool ok = i < we;
-                        const unsigned kk = skey[ok ? i : we - 1];    // slots beyond the range: last entry, zero coefficient
-                        const float av = ok ? sval[i] : 0.f;
-                        const float v2 = (!AN && ok) ? av * __ldg(wsc + (kk >> 10)) : 0.f;
-                        const int m = min(32, we - i0);
-                        for (int j0 = 0; j0 < m; j0 += PF) {
-                            LV fm[PF], fw[AN ? PF : 1];
-#pragma unroll
-                            for (int u = 0; u < PF; ++u) {
-                                const unsigned ku = __shfl_sync(0xffffffffu, kk, j0 + u);
-                                const unsigned po = (ku >> 10) * (unsigned)D;
-                                fm[u] = lv_ldg<VEC>(wmcol_l + po);
-                                if constexpr (AN) fw[u] = lv_ldg<VEC>(wcol_l + po);
-                            }
-#pragma unroll
-                            for (int u = 0; u < PF; ++u) {
-                                const int n = (int)(__shfl_sync(0xffffffffu, kk, j0 + u) & 1023u);
-                                const float a = __shfl_sync(0xffffffffu, av, j0 + u);
-                                if (n != cur_n) {
-                                    if (cur_n >= 0) {
-                                        flush(first_run ? 0 : -1);
-                                        first_run = false;
-                                    }
-                                    cur_n = n;
-                                    xpre = lv_ldg<VEC>(xcol2 + (size_t)n * D);
-                                    gpre = lv_ldcg<VEC>(gcol + (size_t)n * D);
-                                    s1 = lv_zero<VEC>();
-                                    s2v = lv_zero<VEC>();
-                                    s2 = 0.f;
-                                }
-#pragma unroll
-                                for (int i = 0; i < VEC; ++i) s1.v[i] = fmaf(a, fm[u].v[i], s1.v[i]);
-                                if constexpr (AN) {
-#pragma unroll
-                                    for (int i = 0; i < VEC; ++i) s2v.v[i] = fmaf(a, fw[u].v[i], s2v.v[i]);
-                                } else {
-                                    s2 += __shfl_sync(0xffffffffu, v2, j0 + u);
-                                }
-                            }
-                        }
-                    }
-                };
-                if (aniso) walk(std::true_type{}); else walk(std::false_type{});
-                if (cur_n >= 0) flush(first_run ? 0 : 1);
-            }
-            __syncthreads();
-            if (warp == 0) {                                      // merge the parked runs by row, in list order (in place)
-                int j = -1, last = -1;
-                LV acc = lv_zero<VEC>();
-                float a2 = 0.f;
-                for (int i = 0; i < 16; ++i) {
-                    const int n = prow[i];
-                    if (n < 0) continue;
-                    const LV v = lv_ld<VEC>(part + i * DC + dl);
-                    const float p2 = part2[i];
-                    __syncwarp();
-                    if (n != last) { ++j; last = n; acc = lv_zero<VEC>(); a2 = 0.f; }
-#pragma unroll
-                    for (int q = 0; q < VEC; ++q) acc.v[q] += v.v[q];
-                    a2 += p2;
-                    lv_st<VEC>(part + j * DC + dl, acc);
-                    if (lane == 0) { part2[j] = a2; mrow[j] = n; }
-                    __syncwarp();
-                }
-                if (lane == 0) mcount = j + 1;
-            }
-            __syncthreads();
-            for (int j = warp; j < mcount; j += 8) {
-                const int n = mrow[j];
-                const LV xv = lv_ldg<VEC>(xcol2 + (size_t)n * D);
-                LV gv = lv_ldcg<VEC>(gcol + (size_t)n * D);
-                const LV v = lv_ld<VEC>(part + j * DC + dl);
-                const float p2 = part2[j];
-#pragma unroll
-                for (int q = 0; q < VEC; ++q) gv.v[q] += fmaf(-xv.v[q], p2, v.v[q]);
-                if (dok2) lv_st<VEC>(gcol + (size_t)n * D, gv);
-            }
-            __syncthreads();
-            if (threadIdx.x == 0) lcount = 0;
-            __syncthreads();
-        }
-    }
+__global__ void __launch_bounds__(256, VEC == 4 ? 2 : 4) head_bwd_kernel(MGP_HEAD_BWD_PARAMS) {
+    head_bwd_body<VEC, false>(MGP_HEAD_BWD_ARGS);
 }
+
+#undef MGP_HEAD_BWD_PARAMS
+#undef MGP_HEAD_BWD_ARGS
 
 // a17 helper: the training loss on the head's output (ref train_and_test.py:37-41, :55)
 //   loss = CE(out[:,:,0], gt) + mine_coef * mean_{t>=1} CE(out[:,:,t], gt),   CE = mean over the batch
@@ -1013,6 +540,15 @@ extern "C" int mgp_head_select_top1(const uint64_t* best, const float* xhat_nd, 
     return MGP_OK;
 }
 
+int head_bwd_proto_weights(const float* mu, const float* sigma, float* w, float* wm, float* wsc, int* noniso, int P,
+                           int D, cudaStream_t st) {
+    const size_t npd = (size_t)P * D;
+    MGP_CUDA(cudaMemsetAsync(noniso, 0, sizeof(int), st));
+    proto_weight_kernel<<<(unsigned)((npd + 255) / 256), 256, 0, st>>>(mu, sigma, w, wm, wsc, noniso, npd, D);
+    MGP_CHECK_LAUNCH();
+    return MGP_OK;
+}
+
 extern "C" size_t mgp_head_bwd_ws_bytes(int B, int HW, int P, int D) {
     return ((size_t)2 * P * D + (size_t)B * HW * D + (size_t)P + 64) * sizeof(float);
 }
@@ -1034,10 +570,8 @@ extern "C" int mgp_head_bwd_x(const float* grad_logits, const float* logits, con
     float* g_xhat = wm + (size_t)P * D;
     float* wsc = g_xhat + (size_t)B * HW * D;
     int* noniso = reinterpret_cast<int*>(wsc + P);
-    const size_t npd = (size_t)P * D;
-    MGP_CUDA(cudaMemsetAsync(noniso, 0, sizeof(int), st));
-    proto_weight_kernel<<<(unsigned)((npd + 255) / 256), 256, 0, st>>>(mu, sigma, w, wm, wsc, noniso, npd, D);
-    MGP_CHECK_LAUNCH();
+    const int rc = head_bwd_proto_weights(mu, sigma, w, wm, wsc, noniso, P, D, st);
+    if (rc != MGP_OK) return rc;
     // dims per CTA: 32 lanes x 4 (one CTA per image at D = 128: the entry list is built and sorted once) or x 2
     static const bool vec2_forced = getenv("MGP_HEAD_BWD_VEC2") != nullptr;
     const int DC = ((D % 128) == 0 && !vec2_forced) ? 128 : 64;

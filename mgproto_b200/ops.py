@@ -18,7 +18,7 @@ from ._lib import (MGP_MATH_AUTO, MGP_MATH_FP32, MGP_MATH_TC, MGP_MATH_TC_ISO, M
                    MGP_OUT_LOGP_NP, MGP_OUT_NEGP_BPHW, MGP_OUT_TOP1_BP, MGP_X_BF16, MGP_X_F16, MGP_X_F32, MGP_X_NHWC,
                    check)
 
-__all__ = ["normalize_fwd", "logprob", "log_density", "logprob_top1", "head_select", "head_select_top1", "head_level0", "head_forward", "HeadFunction", "mined_gather", "bank_enqueue",
+__all__ = ["normalize_fwd", "logprob", "log_density", "logprob_top1", "head_select", "head_select_top1", "head_select_long", "head_select_top1_long", "head_level0", "head_forward", "head_backward_long", "HeadFunction", "mined_gather", "bank_enqueue",
            "bank_linearize", "bank_shadow_sync", "em_plan", "em_stats", "em_update", "update_gmm", "em_estep", "em_mstep_closed", "em_mstep_div", "topt_pool", "ood_score", "push_argmin", "push_argmin_top1", "push_records", "push_store", "push_merge", "push_assign", "mine_cross_entropy",
            "proxy_anchor", "ProxyAnchorFunction",
            "MATH_MODES"]
@@ -399,6 +399,63 @@ def head_select(logp, weight_cp, gt, T, C, K, B=None, HW=None):
     return logits, vals, idx
 
 
+# ----------------------------------------------------------------------------------- a4-a7 on long maps
+LONG_MAP_HW = 1024          # the head routes maps of more patches than this to the long-map kernels
+LONG_MAP_MAX_HW = 4096      # ... which take up to this many
+
+
+def _top1_long_fits(C, K, D, T):
+    """mgp_head_select_top1_long's shared-memory layout (csrc/head_long.cu, top1_long_layout) leaves room for a slice
+    of at least 32 patches within 200 KB."""
+    head = (2 * C * K + 3 * K * T + K + 3) & ~3
+    return K <= 64 and head + 2 * K * D + 2 * K + 33 * K <= 200 * 1024 // 4
+
+
+@_on_device
+def head_select_long(logp, weight_cp, gt, T, C, K):
+    """head_select on a [B,P,HW] log p at 1 <= HW <= 4096 (mgp_head_select_long): the same outputs, without the
+    1024-patch limit of the register-resident kernels.  -> (logits [B,C,T], vals [B,P,T], idx [B,P,T] int32)."""
+    lp = _req(logp, torch.float32, "logp")
+    w = _req(weight_cp, torch.float32, "last_layer.weight")
+    if lp.dim() != 3:
+        raise RuntimeError("mgproto_b200: head_select_long takes log p as [B,P,HW]")
+    B, P, HW = lp.shape
+    if P != C * K or w.shape != (C, P):
+        raise RuntimeError("mgproto_b200: shape mismatch in head_select_long")
+    if gt is not None:
+        gt = _req(gt, torch.int64, "gt")
+        if gt.shape != (B,):
+            raise RuntimeError("mgproto_b200: gt must be [B]")
+    logits = torch.empty((B, C, T), device=lp.device, dtype=torch.float32)
+    vals = torch.empty((B, P, T), device=lp.device, dtype=torch.float32)
+    idx = torch.empty((B, P, T), device=lp.device, dtype=torch.int32)
+    check(_lib.load().mgp_head_select_long(lp.data_ptr(), w.data_ptr(), _p(gt), logits.data_ptr(), vals.data_ptr(),
+                                           idx.data_ptr(), B, HW, C, K, T, _stream()), "mgp_head_select_long")
+    _count(1)
+    return logits, vals, idx
+
+
+@_on_device
+def head_select_top1_long(best, xhat_nd, mu_pd, sigma_pd, weight_cp, gt, T, C, K, HW):
+    """head_select_top1 at 1 <= HW <= 4096 (mgp_head_select_top1_long): level 0 from the packed max / arg-max, the
+    own class's full top-T from its exact fp32 log p, evaluated in patch slices.  gt = -1 everywhere: the level-0 head."""
+    B, P = best.shape
+    x = _req(xhat_nd, torch.float32, "xhat")
+    D = x.shape[1]
+    gt = _req(gt, torch.int64, "gt")
+    if x.shape[0] != B * HW or P != C * K or gt.shape != (B,):
+        raise RuntimeError("mgproto_b200: shape mismatch in head_select_top1_long")
+    logits = torch.empty((B, C, T), device=x.device, dtype=torch.float32)
+    vals = torch.empty((B, P, T), device=x.device, dtype=torch.float32)
+    idx = torch.empty((B, P, T), device=x.device, dtype=torch.int32)
+    check(_lib.load().mgp_head_select_top1_long(best.data_ptr(), x.data_ptr(), mu_pd.data_ptr(), sigma_pd.data_ptr(),
+                                                weight_cp.data_ptr(), gt.data_ptr(), logits.data_ptr(), vals.data_ptr(),
+                                                idx.data_ptr(), B, HW, C, K, D, T, _stream()),
+          "mgp_head_select_top1_long")
+    _count(1)
+    return logits, vals, idx
+
+
 class HeadFunction(torch.autograd.Function):
     """features [B,D,H,W] -> log mixture evidences [B,C,T] (ref model.py:210-222, :254).
 
@@ -421,8 +478,13 @@ class HeadFunction(torch.autograd.Function):
         sg = sigma_ckd.detach().reshape(C * K, D).contiguous()
         wt = weight_cp.detach().contiguous()
         # the labelled fast path needs the tensor-core kernel and head_top1_kernel's shared-memory layout to fit
-        top1_smem = (2 * C * K + K * T + K * (HW + 1) + 2 * K * D + 2 * K + 4) * 4
-        use_top1 = gt is not None and T <= min(32, HW) and HW <= 1024 and top1_smem <= 200 * 1024
+        # (long maps: head_top1_long_kernel's, whose log p tile is a slice of the map)
+        long_map = HW > LONG_MAP_HW
+        if long_map:
+            use_top1 = gt is not None and T <= min(32, HW) and HW <= LONG_MAP_MAX_HW and _top1_long_fits(C, K, D, T)
+        else:
+            top1_smem = (2 * C * K + K * T + K * (HW + 1) + 2 * K * D + 2 * K + 4) * 4
+            use_top1 = gt is not None and T <= min(32, HW) and HW <= 1024 and top1_smem <= 200 * 1024
         stage = _stage_for_top1(B, HW, C * K, D, sg, math) if use_top1 else None
         if stage is not None:       # one pass: normalise + the fp16 hi/lo operands the max / arg-max kernel reads
             xhat, inv, _, ws1 = normalize_fwd(x_add, stage=stage)
@@ -432,10 +494,11 @@ class HeadFunction(torch.autograd.Function):
             best = logprob_top1(xhat, mu, sg, B, HW, math) if use_top1 else None
         if best is not None:
             # labelled step: log p never reaches HBM (wrong-class prototypes only need their max, ref model.py:218-221)
-            logits, vals, idx = head_select_top1(best, xhat, mu, sg, wt, _req(gt, torch.int64, "gt"), T, C, K, HW)
+            top1 = head_select_top1_long if long_map else head_select_top1
+            logits, vals, idx = top1(best, xhat, mu, sg, wt, _req(gt, torch.int64, "gt"), T, C, K, HW)
         else:
             lp = logprob(xhat, mu, sg, MGP_OUT_LOGP_BPHW, B=B, HW=HW, math=math)   # [B,P,HW]: contiguous rows for the mining
-            logits, vals, idx = head_select(lp, wt, gt, T, C, K)
+            logits, vals, idx = (head_select_long if long_map else head_select)(lp, wt, gt, T, C, K)
         ctx.save_for_backward(logits, vals, idx, wt, gt if gt is not None else torch.empty(0), xhat, inv, mu, sg)
         ctx.has_gt = gt is not None
         ctx.dims = (B, HW, C, K, D, T, H, W)
@@ -450,8 +513,8 @@ class HeadFunction(torch.autograd.Function):
             return (None,) * 7
         logits, vals, idx, wt, gt, xhat, inv, mu, sg = ctx.saved_tensors
         B, HW, C, K, D, T, H, W = ctx.dims
-        gx = head_backward(g_logits, logits, vals, idx, wt, gt if ctx.has_gt else None, xhat, inv, mu, sg, ctx.dims,
-                           ctx.x_fmt)
+        bwd = head_backward_long if HW > LONG_MAP_HW else head_backward
+        gx = bwd(g_logits, logits, vals, idx, wt, gt if ctx.has_gt else None, xhat, inv, mu, sg, ctx.dims, ctx.x_fmt)
         return gx, None, None, None, None, None, None
 
 
@@ -476,6 +539,24 @@ def head_backward(g_logits, logits, vals, idx, wt, gt, xhat, inv, mu, sg, dims, 
     return gx
 
 
+@_on_device
+def head_backward_long(g_logits, logits, vals, idx, wt, gt, xhat, inv, mu, sg, dims, x_fmt=MGP_X_F32):
+    """head_backward for the outputs of head_select_long / head_select_top1_long at 1 <= HW <= 4096
+    (mgp_head_bwd_long_x): the same gradient, as deterministic."""
+    B, HW, C, K, D, T, H, W = dims
+    g = _req(g_logits.contiguous(), torch.float32, "grad_logits")
+    lib = _lib.load()
+    nbytes = lib.mgp_head_bwd_long_ws_bytes(B, HW, C * K, D)
+    ws = torch.empty((nbytes,), device=g.device, dtype=torch.uint8)
+    mf = torch.channels_last if x_fmt & MGP_X_NHWC else torch.contiguous_format
+    gx = torch.empty((B, D, H, W), device=g.device, dtype=_X_DTYPES[x_fmt & ~MGP_X_NHWC], memory_format=mf)
+    check(lib.mgp_head_bwd_long_x(g.data_ptr(), logits.data_ptr(), vals.data_ptr(), idx.data_ptr(), wt.data_ptr(),
+                                  _p(gt), xhat.data_ptr(), inv.data_ptr(), mu.data_ptr(), sg.data_ptr(), ws.data_ptr(),
+                                  nbytes, gx.data_ptr(), int(x_fmt), B, HW, C, K, D, T, _stream()), "mgp_head_bwd_long_x")
+    _count(3)
+    return gx
+
+
 def head_level0(x_add, mu_ckd, sigma_ckd, weight_cp, math="auto"):
     """Level 0 of the unlabelled head, [B,C] = head_forward(..., gt=None)[0][:, :, 0] -- all the reference's test /
     OoD loop reads (train_and_test.py:182-199: output[:, :, 0]).  Uses the max/arg-max epilogue (no log p matrix, no
@@ -487,7 +568,11 @@ def head_level0(x_add, mu_ckd, sigma_ckd, weight_cp, math="auto"):
         mu = mu_ckd.detach().reshape(C * K, D).contiguous()
         sg = sigma_ckd.detach().reshape(C * K, D).contiguous()
         wt = weight_cp.detach().contiguous()
-        fits = HW <= 1024 and (2 * C * K + 2 * K + K * (HW + 1) + 2 * K * D + 2 * K + 4) * 4 <= 200 * 1024
+        long_map = HW > LONG_MAP_HW
+        if long_map:
+            fits = HW <= LONG_MAP_MAX_HW and _top1_long_fits(C, K, D, 1)
+        else:
+            fits = HW <= 1024 and (2 * C * K + 2 * K + K * (HW + 1) + 2 * K * D + 2 * K + 4) * 4 <= 200 * 1024
         stage = _stage_for_top1(B, HW, C * K, D, sg, math) if fits else None
         if stage is not None:
             xhat, _, _, ws1 = normalize_fwd(x_add.detach(), stage=stage)
@@ -497,9 +582,10 @@ def head_level0(x_add, mu_ckd, sigma_ckd, weight_cp, math="auto"):
             best = logprob_top1(xhat, mu, sg, B, HW, math) if fits else None
         if best is None:
             lp = logprob(xhat, mu, sg, MGP_OUT_LOGP_BPHW, B=B, HW=HW, math=math)
-            return head_select(lp, wt, None, 1, C, K)[0][:, :, 0]
+            return (head_select_long if long_map else head_select)(lp, wt, None, 1, C, K)[0][:, :, 0]
         none = torch.full((B,), -1, dtype=torch.int64, device=x_add.device)     # no own class: every class keeps level 0 only
-        return head_select_top1(best, xhat, mu, sg, wt, none, 1, C, K, HW)[0][:, :, 0]
+        top1 = head_select_top1_long if long_map else head_select_top1
+        return top1(best, xhat, mu, sg, wt, none, 1, C, K, HW)[0][:, :, 0]
 
 
 def head_forward(x_add, mu_ckd, sigma_ckd, weight_cp, gt, T, math="auto"):
